@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the PixelSSL sseg SSL-training hot path on B200.
+"""Benchmark of the PixelSSL sseg SSL-training hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W [--config mt|cutmix|gct|cct] [--precision f16x3|f16|tf32x3|tf32|fp32]
+                    [--dump-outputs DIR]
     python bench.py --impl reference --gpus N --steps K --warmup W          (torchrun for N > 1)
 
 Default workload (BASELINE.json configs[1]): Mean-Teacher, DeepLab-v2-ResNet101 OS16, per-GPU batch 16
@@ -16,10 +17,11 @@ Printed JSON line (rank 0), keys as in the task statement:
   value      steps timed with the batches already in HBM (``algorithm._train`` on device batches, log_freq off)
   e2e        ``algorithm.train(data_loader, epoch)`` - the plugin API a PixelSSL user calls - on pinned HOST batches
              with log_freq = 1: H2D of every batch and a D2H read of every step's losses inside the timed region
-  roofline   the DOMINANT kernel: the tcgen05 forward/dgrad convolution.  achieved = algorithmic FLOPs (2*M*K*N per
+  roofline   the DOMINANT kernel: the wgmma forward/dgrad convolution.  achieved = algorithmic FLOPs (2*M*K*N per
              launch) / CUDA-event time of its launches, measured live in an instrumented pass right after the timed
              region (events around ~300 launches per step would perturb ``value``); peak = the measured dense 16-bit
-             tensor throughput of MEASURED_PEAKS.json (sustained figure: the kernel runs inside a long step)
+             tensor throughput of MEASURED_PEAKS.json when present, else the H100 SXM data-sheet figures (989 TFLOP/s
+             dense 16-bit, 3.35 TB/s HBM3)
   roofline_wgrad / roofline_hbm   the same for the wgrad kernel and for the metric kernel of BASELINE.json (fused MSE
              consistency fwd+bwd, 12 B/element, HBM-bound; timed inside the timed steps)
   step_tensor_frac   whole-step algorithmic TFLOP/s over the same tensor peak
@@ -28,7 +30,10 @@ Printed JSON line (rank 0), keys as in the task statement:
   gpu_torch_baseline the reference step written with stock PyTorch ops (oracle port on cuda:0: NCHW, cuDNN TF32
              default, eager) on this GPU - the "reference's 1-GPU PyTorch images/sec" of the north_star target
   cpu_baseline / ``--impl reference``   the CPU oracle port of the reference step (torch CPU fp32, up to 32 host
-             threads) on a bounded sample."""
+             threads) on a bounded sample.
+  --dump-outputs DIR   after the timed steps: what the last timed step computed, as DIR/<name>.npy (losses of the
+             step, a fixed seeded sample of each trained model's updated parameters and BN buffers); the inputs are
+             seeded, so two builds can be compared output for output."""
 import argparse
 import json
 import os
@@ -81,8 +86,8 @@ def measured_peaks():
     path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(path):
         d = json.load(open(path))
-        return d.get('hbm_gbs', 6650.0), d.get('bf16_tflops_sustained', 1400.0), 'measured'
-    return 6650.0, 1590.0, 'fallback'
+        return d.get('hbm_gbs', 3350.0), d.get('bf16_tflops_sustained', 989.0), 'measured'
+    return 3350.0, 989.0, 'H100 SXM data sheet'
 
 
 class ClockSampler:
@@ -336,6 +341,8 @@ def run_engine(args):
 
     sat_log = {}
     ms_dev, ktimes, launches = timed(dev, tag='value')
+    if args.dump_outputs and rank == 0:
+        dump_outputs(st['alg'], args.dump_outputs)
     sat_log['after_value'] = ops.h16_status_sites()
     clocks = clock_rec[0] if clock_rec else None
     ms_e2e, _, _ = timed(host, api=True, tag='e2e')
@@ -378,18 +385,17 @@ def run_engine(args):
     tpath = os.path.join(ROOT, 'profiles', 'kernel_traffic.json')
     if os.path.exists(tpath):
         traffic = json.load(open(tpath))
-    kname = {'f16x3': 'conv_tc_pair_kernel (cta_group::2, layers 3/4) + conv_tc_persist_kernel, kind::f16 x3 (fp16 pairs)',
-             'f16': 'conv_tc_pair_kernel + conv_tc_persist_kernel, kind::f16',
-             'tf32x3': 'conv_tc_persist_kernel, kind::tf32 x3', 'tf32': 'conv_tc_kernel / conv_tc_persist_kernel, kind::tf32'}
+    kname = {'f16x3': 'conv_wg_kernel, wgmma f16 x3 (fp16 pairs)', 'f16': 'conv_wg_kernel, wgmma f16',
+             'tf32x3': 'conv_wg_kernel, wgmma tf32 x3', 'tf32': 'conv_wg_kernel, wgmma tf32'}
     roof = _roofline_from(conv_rec, tf_peak, peak_src, 'forward/dgrad convolution: ' + kname.get(args.precision, ''),
                           traffic=traffic.get('conv_fwd_dram_bytes_per_launch'))
-    roof_wg = _roofline_from(wg_rec, tf_peak, peak_src, 'conv_wgrad_tc_kernel (' + args.precision + ')',
+    roof_wg = _roofline_from(wg_rec, tf_peak, peak_src, 'conv_wgrad_wg_kernel (' + args.precision + ')',
                              traffic=traffic.get('conv_wgrad_dram_bytes_per_launch'))
     mma_per_product = 3 if args.precision in ('f16x3', 'tf32x3') else 1
     for r in (roof, roof_wg):
         if r:
             r['mma_rate_frac'] = r['frac'] * mma_per_product * (2.0 if args.precision in ('tf32', 'tf32x3') else 1.0)
-            r['note'] = ('achieved counts each product once; the fp32-grade modes issue 3 MMAs per product, kind::tf32 '
+            r['note'] = ('achieved counts each product once; the fp32-grade modes issue 3 MMAs per product, tf32 '
                          'runs at half the 16-bit rate: mma_rate_frac = tensor-pipe rate over the same peak')
     n_elem = ubs * NUM_CLASSES * size * size
     k_ms = sum(ktimes) / max(len(ktimes), 1) if ktimes else float('nan')
@@ -410,7 +416,7 @@ def run_engine(args):
         'config': {'workload': workload, 'name': args.config,
                    'global_batch': (lbs + ubs) * world, 'parallelism': 'dp%d' % world,
                    'conv_precision': args.precision, 'weights': 'random init (reference initialisers)',
-                   'l2': 'inputs and activations (>20 GB/step) far exceed the 126 MB L2; no explicit flush'},
+                   'l2': 'inputs and activations (>20 GB/step) far exceed the 50 MB L2; no explicit flush'},
         'e2e': {'value': e2e, 'unit': 'images/s',
                 'h2d_bytes_per_step': (lbs + ubs) * (3 + 1) * size * size * 4, 'd2h_bytes_per_step': 24,
                 'api': 'algorithm.train(data_loader, epoch) on pinned host batches, log_freq=1 (losses read back every step)'},
@@ -420,7 +426,7 @@ def run_engine(args):
         'roofline_wgrad': roof_wg,
         'roofline_hbm': roof_hbm,
         'losses': losses,
-        'pipeline_status': {'tcgen05_watchdog': status[0], 'fp16_pair_saturations': status[1],
+        'pipeline_status': {'conv_watchdog': status[0], 'fp16_pair_saturations': status[1],
                             'saturations_by_site_split_fixed_dyn_bnapply_bndx': ops.h16_status_sites(), 'phases': sat_log},
     }
     if args.config == 'mt':
@@ -450,6 +456,27 @@ def run_engine(args):
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def dump_outputs(alg, out_dir):
+    """What the last timed step handed back to the caller of ``_train``: its losses and the updated models.  The
+    parameter vectors are large, so a fixed seeded sample of 2^20 entries of each model's state is stored."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    losses = {k: float(v) for k, v in alg.meters.values().items() if 'loss' in k}
+    np.save(os.path.join(out_dir, 'losses.npy'), np.array([losses[k] for k in sorted(losses)], dtype=np.float64))
+    with open(os.path.join(out_dir, 'losses.json'), 'w') as f:
+        json.dump(sorted(losses), f)
+    g = torch.Generator().manual_seed(2024)
+    # every model the algorithm trains (MT / CutMix: s_model, t_model; GCT: l_model, r_model, fd_model; CCT: model,
+    # which holds the main network and all auxiliary decoders)
+    for name, model in sorted(alg.models.items()):
+        state = model.state_dict()
+        flat = torch.cat([state[k].detach().reshape(-1).float().cpu() for k in sorted(state)
+                          if state[k].is_floating_point()])
+        idx = torch.randint(0, flat.numel(), (1 << 20,), generator=g)
+        np.save(os.path.join(out_dir, '%s_state_sample.npy' % name), flat[idx].numpy().astype(np.float32))
 
 
 def cpu_reference(steps, warmup, lbs, ubs):
@@ -550,6 +577,8 @@ def main():
     ap.add_argument('--no-gpu-torch-baseline', action='store_true')
     ap.add_argument('--no-alt', action='store_true', help='skip the alt_precision pass')
     ap.add_argument('--no-ddp-check', action='store_true', help='N > 1: skip the data-parallel parity check')
+    ap.add_argument('--dump-outputs', type=str, default=None, metavar='DIR',
+                    help='write what the last timed step computed to DIR/<name>.npy')
     ap.add_argument('--ref-device', type=str, default='cpu', choices=['cpu', 'cuda'],
                     help='--impl reference only: cuda = the oracle port with stock PyTorch ops on cuda:0 (informational)')
     args = ap.parse_args()

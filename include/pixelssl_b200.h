@@ -1,5 +1,5 @@
 /*
- * pixelssl_b200 -- C ABI of the B200-native (sm_100a) hot path of PixelSSL's semantic-segmentation
+ * pixelssl_b200 -- C ABI of the H100-native (sm_90a) hot path of PixelSSL's semantic-segmentation
  * SSL training step.  Plain pointers and sizes, no torch types.  Every pointer is a DEVICE pointer
  * unless the parameter name ends in `_host`.  `stream` is a cudaStream_t passed as void*.
  * Every entry point returns 0 on success or a cudaError_t / negative pxl error code; nothing is
@@ -138,7 +138,7 @@ int pxl_bn_bwd_dx(const float* x, const float* y, const float* dy, const float* 
 /* dgamma_acc / dbeta_acc (both or neither): dgamma_acc[c] += dsums[C+c], dbeta_acc[c] += dsums[c] by the same launch
  * (single-GPU path: dsums are the local sums; replaces pxl_bn_bwd_params + the optimizer-side accumulation). */
 /* fp16-pair variants (csrc/h16_prep.cu) of the BatchNorm launches: the SAME pass that writes y (dx) also, or only
- * (y / dx NULL), writes it as the fp16 pair the next tcgen05 convolution reads, so the pair costs no extra trip
+ * (y / dx NULL), writes it as the fp16 pair the next wgmma convolution reads, so the pair costs no extra trip
  * through HBM.  hi / lo: __half NHWC planes, lo nullable.  Forward: fixed scale `hscale`.  Backward: the reduce
  * launch leaves absmax(dz) in slot[2] (DEVICE float[4], zeroed), the dx launch derives the power-of-two scale from
  * it, max|gamma*invstd| and target_log2, and stores s / 1/s in slot[0] / slot[1].
@@ -181,8 +181,8 @@ int pxl_maxpool3x3s2_bwd(const float* x, const float* y, const float* dy, float*
  *   (terms whose coordinate is not divisible by div or falls outside [0,H)x[0,W) are zero).
  *   forward conv: mul=stride, div=1, dy_t = r*dil - pad.   dgrad: mul=1, div=stride, taps negated,
  *   weights transposed to [Cin][tap][Cout] (pxl_conv_transpose_weights).
- * precision: 0 = fp32 FFMA (exact fp32 accumulate), 1 = tf32 tensor cores (tcgen05), 2 = 3xTF32
- *   error-compensated tcgen05.  Unsupported (shape, precision) combos return PXL_ERR_UNSUPPORTED.
+ * precision: 0 = fp32 FFMA (exact fp32 accumulate), 1 = tf32 tensor cores (wgmma), 2 = 3xTF32
+ *   error-compensated wgmma.  Unsupported (shape, precision) combos return PXL_ERR_UNSUPPORTED.
  * ------------------------------------------------------------------------------------------- */
 typedef struct {
     int N, H, W, Cin;        /* input tensor  */
@@ -199,9 +199,9 @@ int pxl_conv_nhwc(const pxl_conv_geom* geom_host, const int* taps_dydx_host /* 2
 /* dW[co][t][ci] += sum over output pixels of dy[n,oy,ox,co] * in[n, iy, ix, ci]   (accumulates) */
 int pxl_conv_wgrad_nhwc(const pxl_conv_geom* geom_host, const int* taps_dydx_host,
                         const float* in, const float* dy, float* dw, void* stream);
-/* tcgen05 path with explicit operands.  precision 1: in_lo / w_lo ignored (NULL).  precision 2
+/* wgmma path with explicit operands.  precision 1: in_lo / w_lo ignored (NULL).  precision 2
  * (3xTF32): in_hi/in_lo and w_hi/w_lo are the tf32 split of the fp32 tensors (pxl_split_tf32):
- * out = in_hi*w_hi + in_lo*w_hi + in_hi*w_lo accumulated in fp32 (TMEM).  Supports mul == div == 1
+ * out = in_hi*w_hi + in_lo*w_hi + in_hi*w_lo accumulated in fp32 (registers).  Supports mul == div == 1
  * and Cin % 32 == 0; anything else returns PXL_ERR_UNSUPPORTED. */
 int pxl_conv_tc_launch(const pxl_conv_geom* geom_host, const int* taps_dydx_host, const float* in_hi,
                        const float* in_lo, const float* w_hi, const float* w_lo, const float* bias,
@@ -226,13 +226,13 @@ typedef struct {
 int pxl_conv_tc_launch_ex(const pxl_conv_geom* geom_host, const int* taps_dydx_host, const pxl_conv_tc_ext* ext_host,
                           const float* in_hi, const float* in_lo, const float* w_hi, const float* w_lo,
                           const float* bias, float* out, void* stream);
-/* tcgen05 wgrad (accumulates into dw): both operands MN-major via TMA, split over the pixel range,
+/* wgmma wgrad (accumulates into dw): both operands MN-major via TMA, split over the pixel range,
  * fp32 RED epilogue.  Same precision / operand convention as pxl_conv_tc_launch; needs mul == div == 1,
  * Cin % 32 == 0 and ldo % 32 == 0. */
 int pxl_conv_wgrad_tc_launch(const pxl_conv_geom* geom_host, const int* taps_dydx_host, const float* in_hi,
                              const float* in_lo, const float* dy_hi, const float* dy_lo, float* dw,
                              void* stream);
-/* ---- fp16 pairs: the operand format of the kind::f16 tcgen05 path (csrc/h16_prep.cu) -------------------------
+/* ---- fp16 pairs: the operand format of the wgmma f16 path (csrc/h16_prep.cu) -------------------------
  * x*s = hi + lo, hi = fp16(x*s), lo = fp16(x*s - hi), s a power of two.  precision 3 ("f16x3"): hi*hi + lo*hi +
  * hi*lo in fp32 (products good to ~2^-21: fp32-grade, like 3xTF32, at twice its MMA rate); precision 4 ("f16"):
  * hi*hi only (11-bit significands = the TF32 numerics of the reference's cuDNN path).  Same geometry contract as
@@ -386,7 +386,7 @@ int pxl_peer_allreduce_bn(double* sums, int n, void* const* mailboxes, int rank,
                           void* stream);
 int pxl_peer_status(void);
 
-/* stem im2col written directly as the fp16 pair [pixels][192] of the kind::f16 path (hi, lo nullable; value*scale) */
+/* stem im2col written directly as the fp16 pair [pixels][192] of the f16 wgmma path (hi, lo nullable; value*scale) */
 int pxl_stem_im2col_h16(const float* img_planar, void* hi, void* lo, float scale, int N, int H, int W, int OH, int OW,
                         void* stream);
 

@@ -633,11 +633,152 @@ def golden_fp64():
     print('fp64 truth written')
 
 
+def parser_table(parser, with_options=True):
+    """argparse options as JSON-comparable rows: dest -> [default, type name, choices(, option strings)]"""
+    import json
+    rows = {}
+    for a in parser._actions:
+        if a.dest == 'help':
+            continue
+        row = [a.default, getattr(a.type, '__name__', a.type), a.choices]
+        if with_options:
+            row.append(list(a.option_strings))
+        rows[a.dest] = row
+    return json.loads(json.dumps(rows, default=str))
+
+
+def array_digest(a):
+    """sha256 over dtype, shape and bytes: equal digests <=> bit-identical arrays"""
+    import hashlib
+    a = np.ascontiguousarray(a)
+    return hashlib.sha256(('%s%s' % (a.dtype.str, a.shape)).encode() + a.tobytes()).hexdigest()
+
+
+HOST_MODELS = [('deeplabv2', 'resnet101'), ('pspnet', 'resnet50'), ('pspnet', 'resnet101')]
+HOST_ALGS = ['ssl_null', 'ssl_mt', 'ssl_cutmix', 'ssl_adv', 'ssl_gct', 'ssl_cct']
+HOST_LRERS = ['steplr', 'multisteplr', 'exponentiallr', 'cosineannealinglr', 'polynomiallr']
+HOST_VAL_CASES = [(37, 53, 33, True), (64, 41, 48, True), (30, 30, 30, True), (45, 70, 0, False)]
+
+
+def golden_host(pixelssl, sseg_proxy):
+    """What the host-side tests compare the engine with (tests/test_host_cpu.py, tests/test_oracle_golden.py): the
+    reference's plugin registry and sampler stream, model state_dict layout and LR groups, checkpoint keys, parser
+    options, LR trajectories, optimizer hyper-parameters, argument validation, TaskFunc hooks and the validation
+    input transforms."""
+    import argparse
+    import gzip
+    import importlib
+    import json
+    import re
+    import types
+    from PIL import Image
+    sys.path.insert(0, os.path.join(REF, 'task', 'sseg'))
+    from pixelssl_b200 import runner
+    rec = {}
+    # sampler stream of the reference's TwoStreamBatchSampler (np.random.seed(5)) and its parser builder
+    np.random.seed(5)
+    rec['sampler_seed5'] = [list(map(int, b)) for b in pixelssl.nn.data.TwoStreamBatchSampler(list(range(9)), list(range(50, 83)), 2, 3)]
+    rec['ssl_algorithms'] = list(pixelssl.ssl_algorithm.SSL_ALGORITHMS)
+    # task models: state_dict layout and LR groups
+    ref_model = importlib.import_module('model')
+    rec['models'] = {}
+    for name, backbone in HOST_MODELS:
+        args = runner.build_args({'ssl_algorithm': 'ssl_null', 'lr': 0.00025, 'momentum': 0.9, 'weight_decay': 0.0005,
+                                  'epochs': 2, 'batch_size': 2, 'unlabeled_batch_size': 0, 'ignore_unlabeled': True,
+                                  'backbone': backbone}, iters_per_epoch=5)
+        ref = getattr(ref_model, name)()(args)
+        rid = {id(p): n for n, p in ref.named_parameters()}
+        rec['models']['%s-%s' % (name, backbone)] = {
+            'state': [[k, list(v.shape), str(v.dtype)] for k, v in ref.state_dict().items()],
+            'param_groups': [[g['lr'], [rid[id(p)] for p in g['params']]] for g in ref.param_groups]}
+    # checkpoint keys of every algorithm's _save_checkpoint
+    rec['checkpoint_keys'] = {}
+    for alg in HOST_ALGS:
+        src = open(os.path.join(REF, 'pixelssl', 'ssl_algorithm', '%s.py' % alg)).read()
+        body = src[src.index('def _save_checkpoint'):]
+        body = body[body.index('state = {'):]
+        body = body[:body.index('}') + 1]
+        rec['checkpoint_keys'][alg] = sorted(set(re.findall(r"'([a-z_]+)'\s*:", body)))
+    # parser options of every algorithm module, and of runner + sseg proxy
+    rec['alg_parser'] = {}
+    for alg in HOST_ALGS:
+        pr = argparse.ArgumentParser()
+        importlib.import_module('pixelssl.ssl_algorithm.' + alg).add_parser_arguments(pr)
+        rec['alg_parser'][alg] = parser_table(pr)
+    pr = pixelssl.runner.create_parser('ssl_null')
+    sseg_proxy.add_parser_arguments(pr)
+    rec['full_parser'] = parser_table(pr, with_options=False)
+    # LR trajectories of every lrer export on a toy two-group optimizer
+    rec['lrer'] = {}
+    for name in HOST_LRERS:
+        parser = argparse.ArgumentParser()
+        pixelssl.nn.lrer.add_parser_arguments(parser)
+        args = parser.parse_args([])
+        args.epochs, args.iters_per_epoch = 6, 4
+        w = [torch.nn.Parameter(torch.zeros(2)), torch.nn.Parameter(torch.zeros(2))]
+        opt = torch.optim.SGD([{'params': [w[0]], 'lr': 0.1}, {'params': [w[1]], 'lr': 1.0}], lr=0.1, momentum=0.9)
+        sched = getattr(pixelssl.nn.lrer, name)(args)(opt)
+        traj = []
+        for _ in range(args.epochs * args.iters_per_epoch - 1 if name == 'polynomiallr' else args.epochs):
+            traj.append([g['lr'] for g in opt.param_groups])
+            opt.step()
+            sched.step()
+        rec['lrer'][name] = traj
+    # optimizer exports: class and per-group hyper-parameters
+    rec['optimizer'] = {}
+    for name in ('sgd', 'adam'):
+        parser = argparse.ArgumentParser()
+        pixelssl.nn.optimizer.add_parser_arguments(parser)
+        args = parser.parse_args(['--lr', '0.00025'])
+        w = [torch.nn.Parameter(torch.zeros(2)), torch.nn.Parameter(torch.zeros(3))]
+        opt = getattr(pixelssl.nn.optimizer, name)(args)([{'params': [w[0]], 'lr': args.lr}, {'params': [w[1]], 'lr': 10 * args.lr}])
+        rec['optimizer'][name] = {'class': type(opt).__module__ + '.' + type(opt).__name__,
+                                  'groups': json.loads(json.dumps([{k: v for k, v in g.items() if k != 'params'}
+                                                                   for g in opt.param_groups], default=str))}
+    # argument validation of every algorithm constructor (the cases of tests/test_host_cpu.py)
+    sys.path.insert(0, os.path.join(ROOT, 'tests'))
+    import test_host_cpu as T
+    rec['constructor_rejects'] = []
+    cls = {'ssl_mt': 'SSLMT', 'ssl_cutmix': 'SSLCUTMIX', 'ssl_adv': 'SSLADV', 'ssl_gct': 'SSLGCT', 'ssl_cct': 'SSLCCT'}
+    for alg, override in T._CASES:
+        cfg = dict(T._BASE_CFG, ssl_algorithm=alg, **T._VALID[alg])
+        cfg.update(override or {})
+        try:
+            getattr(importlib.import_module('pixelssl.ssl_algorithm.' + alg), cls[alg])(runner.build_args(dict(cfg), iters_per_epoch=5))
+            rejected = False
+        except SystemExit:
+            rejected = True
+        rec['constructor_rejects'].append([alg, override, rejected])
+    # TaskFunc shape hooks
+    rec['task_func'] = {}
+    for arch in ('deeplabv2', 'pspnet'):
+        args = runner.build_args(dict(T._BASE_CFG, ssl_algorithm='ssl_cct', models={'model': arch}, im_size=65, **T._VALID['ssl_cct']),
+                                 iters_per_epoch=5)
+        ref = importlib.import_module('func').task_func()(args)
+        rec['task_func'][arch] = {h: getattr(ref, h)() for h in T.TASK_FUNC_HOOKS}
+        rec['task_func'][arch]['METRIC_STR'] = ref.METRIC_STR
+    # validation transforms (_val_prehandle) on seeded images: digests of the exact output arrays
+    sseg_data = importlib.import_module('data')
+    rec['val_prehandle'] = {}
+    for h, w, size, rescaling in HOST_VAL_CASES:
+        rs = np.random.RandomState(h * 100 + w)
+        img = rs.randint(0, 256, (h, w, 3)).astype(np.uint8)
+        lab = rs.randint(0, 21, (h, w)).astype(np.uint8)
+        fake = types.SimpleNamespace(args=types.SimpleNamespace(val_rescaling=rescaling, im_size=size),
+                                     IMAGE=sseg_data.PascalVocDataset.IMAGE, LABEL=sseg_data.PascalVocDataset.LABEL)
+        x, y = sseg_data.PascalVocDataset._val_prehandle(fake, Image.fromarray(img), Image.fromarray(lab))
+        rec['val_prehandle']['%d_%d_%d_%d' % (h, w, size, rescaling)] = [array_digest(x.numpy()), array_digest(y.numpy())]
+    with gzip.open(os.path.join(OUT, 'host_reference.json.gz'), 'wt') as f:
+        json.dump(rec, f, sort_keys=True)
+    print('host reference records written')
+
+
 if __name__ == '__main__':
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(os.cpu_count())
     pixelssl, sseg_proxy = patch_and_import()
-    which = sys.argv[1:] or ['ops', 'forward', 'mt', 'nullcutmix', 'adv', 's4l', 'gct', 'cct', 'pspnet', 'val', 'input', 'fp64']
+    which = sys.argv[1:] or ['ops', 'forward', 'mt', 'nullcutmix', 'adv', 's4l', 'gct', 'cct', 'pspnet', 'val', 'input', 'fp64',
+                             'host']
     if which == ['fp64']:
         golden_fp64()
         sys.exit(0)
@@ -675,3 +816,5 @@ if __name__ == '__main__':
         golden_input(pixelssl, sseg_proxy)
     if 'fp64' in which:
         golden_fp64()
+    if 'host' in which:
+        golden_host(pixelssl, sseg_proxy)

@@ -1,4 +1,4 @@
-"""pixelssl_b200: B200-native (sm_100a) engine for PixelSSL's semantic-segmentation SSL training
+"""pixelssl_b200: H100-native (sm_90a) engine for PixelSSL's semantic-segmentation SSL training
 step, exposed behind PixelSSL's own ``ssl_algorithm`` / ``task_template`` plugin API.
 
     import pixelssl, pixelssl_b200

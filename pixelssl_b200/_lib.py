@@ -143,7 +143,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             'pixelssl_b200: %s not found. Build it with `python -c "import __graft_entry__ as g; '
-            'g.build()"` (nvcc, sm_100a). There is no CPU/PyTorch fallback.' % LIB_PATH)
+            'g.build()"` (nvcc, sm_90a). There is no CPU/PyTorch fallback.' % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)          # AttributeError if the symbol is missing: loud by design

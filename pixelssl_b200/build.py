@@ -1,4 +1,4 @@
-"""Builds libpixelssl_b200.so (sm_100a only) in-tree with nvcc.  No torch headers involved: the
+"""Builds libpixelssl_b200.so (sm_90a only) in-tree with nvcc.  No torch headers involved: the
 library is a plain C-ABI shared object (include/pixelssl_b200.h)."""
 import os
 import subprocess
@@ -10,7 +10,7 @@ LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'libpixelssl_b200.so')
 SOURCES = ['loss_kernels.cu', 'norm_pool_optim.cu', 'resample.cu', 'conv_fp32.cu', 'conv_tc.cu',
            'h16_prep.cu', 'conv_api.cu', 'gct_kernels.cu', 'metrics_noise.cu', 'peer_exchange.cu', 'input_pipeline.cu', 'aspp_gather.cu', 's4l_kernels.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '--use_fast_math=false']
 
 
@@ -51,7 +51,7 @@ def build(force=False, verbose=True):
             raise RuntimeError('nvcc failed on %s:\n%s' % (src, out.decode()))
         if verbose and out.strip():
             print(out.decode())
-    cmd = [_nvcc(), '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a']
+    cmd = [_nvcc(), '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a']
     subprocess.check_call(cmd)
     return LIB
 

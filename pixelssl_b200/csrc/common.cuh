@@ -1,12 +1,20 @@
-// Shared helpers for the pixelssl_b200 sm_100a kernels.
+// Shared helpers for the pixelssl_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "../../include/pixelssl_b200.h"
 
-#define PXL_NUM_SMS 148
+#define PXL_NUM_SMS 132
 
 extern "C" void pxl_count_launch_(int n);
+
+// per-(purpose, stream) scratch buffer (conv_api.cu); *rc != 0 on failure
+#define PXL_WS_WGRAD 0
+#define PXL_WS_BIAS 1
+#define PXL_WS_CE 2
+#define PXL_WS_PURPOSES 3
+#define PXL_WS_STREAMS 8
+extern "C" void* pxl_workspace_(int purpose, void* stream, size_t bytes, int* rc);
 
 #define PXL_CHECK_LAUNCH()                                   \
     do {                                                     \
@@ -20,8 +28,8 @@ static inline int64_t pxl_cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 // Programmatic dependent launch (PDL): a kernel launched through pxl_launch_pdl may become resident while its
 // predecessor in the stream is still running (as SM resources free up); it must execute PXL_PDL_SYNC() before it
 // touches global memory - the predecessor's results are complete and visible after it.  What overlaps is the launch
-// latency, CTA scheduling and the part of the kernel before PXL_PDL_SYNC (barrier init, TMEM allocation, shared
-// memory clearing of the tcgen05 kernels).  PXL_PDL=0 launches everything with plain stream order.
+// latency, CTA scheduling and the part of the kernel before PXL_PDL_SYNC (barrier init, shared
+// memory clearing of the wgmma kernels).  PXL_PDL=0 launches everything with plain stream order.
 #define PXL_PDL_SYNC()                                                   \
     do {                                                                 \
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  \

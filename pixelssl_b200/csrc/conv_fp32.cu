@@ -1,7 +1,7 @@
 // FP32 (FFMA, exact fp32 accumulate) implicit-GEMM convolution on NHWC activations with a tap
 // table: forward, dgrad (same kernel, transposed weights + negated taps), wgrad (split-K with
 // fp32 atomics), weight transpose, bias gradient and the 7x7/2 stem.  This is the precise path
-// (precision == 0) and the fallback for shapes the tcgen05 kernels do not cover.
+// (precision == 0) and the fallback for shapes the wgmma kernels do not cover.
 //
 // GEMM view:  out[M = N*OH*OW, Cout] = A[M, K = ntaps*Cin] * W^T[K, Cout], A gathered on the fly
 // (im2col-free): row m, k = (tap, ci) reads in[n, (oy*mul+dy_t)/div, (ox*mul+dx_t)/div, ci].
@@ -417,10 +417,11 @@ extern "C" int pxl_conv_transpose_weights_batched(const float* src_base, float* 
 }
 
 // ------------------------------------------------------------------------------------------
-// bias gradient: dbias[co] (+)= sum_rows dy[row*ldo + co]
+// bias gradient: dbias[co] (+)= sum_rows dy[row*ldo + co].  Each block stores its partial sums; a second kernel adds
+// them in block order, so the result does not depend on the order in which blocks finish.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-bias_grad_kernel(const float* __restrict__ dy, int64_t rows, int Cout, int ldo, int64_t rowsPerBlock, float* __restrict__ dbias) {
+bias_grad_kernel(const float* __restrict__ dy, int64_t rows, int Cout, int ldo, int64_t rowsPerBlock, float* __restrict__ part) {
     // thread (c = tid % 32, r = tid / 32); Cout <= 32 per grid.y slice
     const int c = blockIdx.y * 32 + (threadIdx.x & 31), rl = threadIdx.x >> 5;
     const int64_t r0 = (int64_t)blockIdx.x * rowsPerBlock, r1 = min(rows, r0 + rowsPerBlock);
@@ -434,8 +435,17 @@ bias_grad_kernel(const float* __restrict__ dy, int64_t rows, int Cout, int ldo, 
         float t = 0.f;
 #pragma unroll
         for (int i = 0; i < 8; ++i) t += sm[i][threadIdx.x & 31];
-        atomicAdd(dbias + c, t);
+        part[(int64_t)blockIdx.x * Cout + c] = t;
     }
+}
+
+__global__ void __launch_bounds__(256)
+bias_grad_sum_kernel(const float* __restrict__ part, int nblk, int Cout, float* __restrict__ dbias) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= Cout) return;
+    float s = 0.f;
+    for (int b = 0; b < nblk; ++b) s += __ldg(part + (int64_t)b * Cout + c);
+    dbias[c] += s;
 }
 
 extern "C" int pxl_bias_grad(const float* dy, int64_t rows, int Cout, int ldo, float* dbias, int accumulate, void* stream) {
@@ -448,7 +458,12 @@ extern "C" int pxl_bias_grad(const float* dy, int64_t rows, int Cout, int ldo, f
     int64_t rb = pxl_cdiv(rows, PXL_NUM_SMS * 4);
     if (rb < 64) rb = 64;
     dim3 grid((unsigned)pxl_cdiv(rows, rb), (unsigned)pxl_cdiv(Cout, 32));
-    bias_grad_kernel<<<grid, 256, 0, st>>>(dy, rows, Cout, ldo, rb, dbias);
+    int rc = 0;
+    float* part = (float*)pxl_workspace_(PXL_WS_BIAS, stream, (size_t)grid.x * Cout * sizeof(float), &rc);
+    if (rc) return rc;
+    bias_grad_kernel<<<grid, 256, 0, st>>>(dy, rows, Cout, ldo, rb, part);
+    PXL_CHECK_LAUNCH();
+    bias_grad_sum_kernel<<<(unsigned)pxl_cdiv(Cout, 256), 256, 0, st>>>(part, (int)grid.x, Cout, dbias);
     PXL_CHECK_LAUNCH();
     return 0;
 }
@@ -596,7 +611,7 @@ extern "C" int pxl_stem_conv7x7s2_wgrad(const float* img, const float* dy, float
 // ------------------------------------------------------------------------------------------
 // stem im2col for the tensor-core path: cols[pixel][k], k = (r*7 + s)*3 + c for k < 147 (the physical
 // order of the channels_last [64,3,7,7] weight), zero for 147 <= k < 160.  The 7x7/2 stem then runs as a
-// flat 1x1 convolution with 160 input lanes on tcgen05 (forward and wgrad share the matrix).
+// flat 1x1 convolution with 160 input lanes on wgmma (forward and wgrad share the matrix).
 // ------------------------------------------------------------------------------------------
 #define ST_KP 160
 __global__ void __launch_bounds__(256)
@@ -632,7 +647,7 @@ extern "C" int pxl_stem_im2col(const float* img, float* cols, int N, int H, int 
     return 0;
 }
 
-// fp16-pair variant for the kind::f16 tensor-core path (csrc/h16_prep.cu): the unfolded stem matrix is written directly
+// fp16-pair variant for the f16 wgmma tensor-core path (csrc/h16_prep.cu): the unfolded stem matrix is written directly
 // as hi / lo planes [pixels][192] (147 taps*channels + 45 zero lanes: K must be a multiple of the 64-element operand
 // row), value * scale = hi + lo.  768 B per output pixel instead of 640 B of fp32, and no separate split pass.
 #include <cuda_fp16.h>
@@ -651,7 +666,7 @@ stem_im2col_h16_kernel(const float* __restrict__ img, uint2* __restrict__ hi, ui
                        int N, int H, int W, int OH, int OW, int tilesX, int tilesY, int* __restrict__ sat) {
     __shared__ float patch[3 * IM_PH * IM_PW];
     __shared__ short koff_s[ST_KH];          // the lanes of a warp index the table with 32 different k: from constant memory
-                                             // that serialises 32-fold (it bounded the kernel: 1.57 ms -> see profiles/)
+                                             // that serialises 32-fold
     for (int i = threadIdx.x; i < ST_KH; i += blockDim.x) koff_s[i] = (short)c_im_koff[i];
     const int t = blockIdx.x;
     const int tx = t % tilesX, ty = (t / tilesX) % tilesY, n = t / (tilesX * tilesY);

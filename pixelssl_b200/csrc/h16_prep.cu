@@ -1,10 +1,10 @@
-// fp16 "pairs": the operand format of the kind::f16 tcgen05 convolutions (conv_tc.cu, precision 3 / 4).
+// fp16 "pairs": the operand format of the wgmma f16 convolutions (conv_tc.cu, precision 3 / 4).
 //
 //   t  = x * s                 s = a power of two (exact), per tensor
 //   hi = fp16_rn(t)            11 significant bits
 //   lo = fp16_rn(t - hi)       the next 11 bits (t - hi is exact in fp32)
 //
-// so x*s = hi + lo up to max(2^-22 |t|, 2^-25): with hi*hi + lo*hi + hi*lo accumulated in fp32 (TMEM) a product
+// so x*s = hi + lo up to max(2^-22 |t|, 2^-25): with hi*hi + lo*hi + hi*lo accumulated in fp32 a product
 // carries a relative error of ~2^-21, the level of the 3xTF32 path, at twice its MMA rate and with no in-kernel
 // operand transform; hi alone has the 11-bit significand of TF32.  fp16's narrow exponent is what the scale is
 // for: activations and weights use fixed powers of two chosen by the caller, gradients a per-tensor scale derived

@@ -22,7 +22,7 @@ extern "C" void pxl_reset_launch_count(void) { g_launches = 0; }
 // ------------------------------------------------------------------------------------------
 // MSE consistency  (ssl_mt.py:115,179-187)
 //   algorithmic traffic: read s, read t (8 B/elem) [+ write grad (4 B/elem)]
-//   design: persistent grid = 148 SMs x 4 CTAs x 256 threads, 128-bit streaming loads, 4-deep
+//   design: persistent grid = PXL_NUM_SMS x 4 CTAs x 256 threads, 128-bit streaming loads, 4-deep
 //   unroll (8 independent LDG.128 in flight per thread), warp-shuffle + smem block reduction,
 //   fp64 per-block partials, last-block-done deterministic final sum.
 // ------------------------------------------------------------------------------------------
@@ -191,7 +191,7 @@ extern "C" int pxl_mse_consistency_bwd(const float* s, const float* t, int64_t n
 template <bool WRITE_GRAD>
 __global__ void __launch_bounds__(256)
 ce2d_kernel(const float* __restrict__ logits, const float* __restrict__ labels, int C, int64_t HW,
-            int ignore_index, float* __restrict__ per_sample, float* __restrict__ grad,
+            int ignore_index, float* __restrict__ part, float* __restrict__ grad,
             const float* __restrict__ upstream, float upstream_const) {
     const int b = blockIdx.y;
     const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -238,8 +238,18 @@ ce2d_kernel(const float* __restrict__ logits, const float* __restrict__ labels, 
         float s = 0.f;
 #pragma unroll
         for (int i = 0; i < 8; ++i) s += wp[i];
-        atomicAdd(per_sample + b, s / (float)HW);
+        part[(int64_t)b * gridDim.x + blockIdx.x] = s / (float)HW;
     }
+}
+
+// per_sample[b] = sum of the blocks' partials in block order (no dependence on the order blocks finish)
+__global__ void __launch_bounds__(128)
+ce2d_sum_kernel(const float* __restrict__ part, int nblk, int n, float* __restrict__ per_sample) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= n) return;
+    float s = 0.f;
+    for (int k = 0; k < nblk; ++k) s += __ldg(part + (int64_t)b * nblk + k);
+    per_sample[b] = s;
 }
 
 extern "C" int pxl_ce2d(const float* logits, const float* labels, int n, int C, int64_t HW,
@@ -248,11 +258,14 @@ extern "C" int pxl_ce2d(const float* logits, const float* labels, int n, int C, 
     if (!logits || !labels || !per_sample || n <= 0 || C <= 0 || HW <= 0) return PXL_ERR_BAD_ARG;
     if (C > CE_MAXC) return PXL_ERR_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = cudaMemsetAsync(per_sample, 0, sizeof(float) * n, st);
-    if (e != cudaSuccess) return (int)e;
     dim3 grid((unsigned)pxl_cdiv(HW, 256), (unsigned)n);
-    if (grad_logits) ce2d_kernel<true><<<grid, 256, 0, st>>>(logits, labels, C, HW, ignore_index, per_sample, grad_logits, upstream, upstream_const);
-    else ce2d_kernel<false><<<grid, 256, 0, st>>>(logits, labels, C, HW, ignore_index, per_sample, nullptr, nullptr, 0.f);
+    int rc = 0;
+    float* part = (float*)pxl_workspace_(PXL_WS_CE, stream, (size_t)grid.x * n * sizeof(float), &rc);
+    if (rc) return rc;
+    if (grad_logits) ce2d_kernel<true><<<grid, 256, 0, st>>>(logits, labels, C, HW, ignore_index, part, grad_logits, upstream, upstream_const);
+    else ce2d_kernel<false><<<grid, 256, 0, st>>>(logits, labels, C, HW, ignore_index, part, nullptr, nullptr, 0.f);
+    PXL_CHECK_LAUNCH();
+    ce2d_sum_kernel<<<(unsigned)pxl_cdiv(n, 128), 128, 0, st>>>(part, (int)grid.x, n, per_sample);
     PXL_CHECK_LAUNCH();
     return 0;
 }

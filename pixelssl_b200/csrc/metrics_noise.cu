@@ -49,7 +49,7 @@ extern "C" int pxl_confusion_matrix(const float* pred, const float* gt, int n, i
     if (!pred || !gt || !cmat || n <= 0 || C <= 0 || HW <= 0) return PXL_ERR_BAD_ARG;
     if (C > CM_MAX_CLASSES || n > 65535) return PXL_ERR_UNSUPPORTED;
     int bx = (int)pxl_cdiv(HW, 256 * 4);
-    const int cap = pxl_cdiv(148 * 8, n) > 1 ? (int)pxl_cdiv(148 * 8, n) : 1;
+    const int cap = pxl_cdiv(PXL_NUM_SMS * 8, n) > 1 ? (int)pxl_cdiv(PXL_NUM_SMS * 8, n) : 1;
     if (bx > cap) bx = cap;
     dim3 grid((unsigned)bx, (unsigned)n);
     confusion_kernel<<<grid, 256, (size_t)C * C * sizeof(unsigned int), (cudaStream_t)stream>>>(
@@ -120,7 +120,7 @@ extern "C" int pxl_gaussian_noise(float* inp, const float* noise, int n, int64_t
     gn_minmax_kernel<<<dim3((unsigned)chunks, (unsigned)n), 256, 0, st>>>(inp, CHW, workspace);
     PXL_CHECK_LAUNCH();
     int bx = (int)pxl_cdiv(CHW, 256 * 4);
-    const int cap = pxl_cdiv(148 * 8, n) > 1 ? (int)pxl_cdiv(148 * 8, n) : 1;
+    const int cap = pxl_cdiv(PXL_NUM_SMS * 8, n) > 1 ? (int)pxl_cdiv(PXL_NUM_SMS * 8, n) : 1;
     if (bx > cap) bx = cap;
     gn_apply_kernel<<<dim3((unsigned)bx, (unsigned)n), 256, 0, st>>>(inp, noise, CHW, workspace, chunks);
     PXL_CHECK_LAUNCH();

@@ -20,7 +20,7 @@ static RedLayout red_layout(int64_t rows, int C) {
     L.colBlocks = (int)pxl_cdiv(c4, L.TX);
     // 8 CTAs per SM in total, but every CTA ends with 2 fp64 atomics per channel: cap the row blocks (= atomics per
     // address) at one per 256 KB of tensor, at least one per SM - on a 17 MB layer ~550 contended atomics per
-    // address cost more than streaming the layer (tools/bench_bn.py: 45 us vs 20 us)
+    // address can cost more than streaming the layer (tools/bench_bn.py)
     int64_t target = (int64_t)PXL_NUM_SMS * 8 / L.colBlocks;
     int64_t cap = rows * C / 65536;
     if (cap < PXL_NUM_SMS) cap = PXL_NUM_SMS;
@@ -697,15 +697,19 @@ extern "C" int pxl_maxpool3x3s2_fwd(const float* x, float* y, int N, int H, int 
 
 __global__ void __launch_bounds__(256)
 maxpool_bwd_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dx,
-                   int N, int H, int W, int C, int OH, int OW) {
-    const int64_t total = (int64_t)N * OH * OW * C;
+                   int N, int H, int W, int C, int OH, int OW, int py, int px) {
+    // outputs (oy, ox) with oy % 2 == py and ox % 2 == px: their 3x3 / stride-2 windows are disjoint, so each
+    // input element receives at most one gradient per launch and a plain add suffices
+    const int QH = (OH - py + 1) / 2, QW = (OW - px + 1) / 2;
+    const int64_t total = (int64_t)N * QH * QW * C;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
-        const int c = (int)(i % C);
-        int64_t p = i / C;
-        const int ox = (int)(p % OW); p /= OW;
-        const int oy = (int)(p % OH);
-        const int n = (int)(p / OH);
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += stride) {
+        const int c = (int)(k % C);
+        int64_t p = k / C;
+        const int ox = 2 * (int)(p % QW) + px; p /= QW;
+        const int oy = 2 * (int)(p % QH) + py;
+        const int n = (int)(p / QH);
+        const int64_t i = ((int64_t)(n * OH + oy) * OW + ox) * C + c;
         float m = -CUDART_INF_F;
         int64_t arg = -1;
 #pragma unroll
@@ -721,7 +725,7 @@ maxpool_bwd_kernel(const float* __restrict__ x, const float* __restrict__ dy, fl
                 if (arg < 0 || v > m || isnan(v)) { m = v; arg = idx; }
             }
         }
-        if (arg >= 0) atomicAdd(dx + arg, __ldg(dy + i));
+        if (arg >= 0) dx[arg] += __ldg(dy + i);
     }
 }
 
@@ -732,10 +736,16 @@ extern "C" int pxl_maxpool3x3s2_bwd(const float* x, const float* y, const float*
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaMemsetAsync(dx, 0, sizeof(float) * (size_t)N * H * W * C, st);
     if (e != cudaSuccess) return (int)e;
-    const int64_t total = (int64_t)N * OH * OW * C;
-    int blocks = (int)(pxl_cdiv(total, 256) < PXL_NUM_SMS * 16 ? pxl_cdiv(total, 256) : PXL_NUM_SMS * 16);
-    maxpool_bwd_kernel<<<blocks, 256, 0, st>>>(x, dy, dx, N, H, W, C, OH, OW);
-    PXL_CHECK_LAUNCH();
+    // four parity classes in a fixed order: windows overlap only across classes, so no atomics and the sums do not
+    // depend on timing
+    for (int cls = 0; cls < 4; ++cls) {
+        const int py = cls >> 1, px = cls & 1;
+        const int64_t total = (int64_t)N * ((OH - py + 1) / 2) * ((OW - px + 1) / 2) * C;
+        if (total <= 0) continue;
+        int blocks = (int)(pxl_cdiv(total, 256) < PXL_NUM_SMS * 16 ? pxl_cdiv(total, 256) : PXL_NUM_SMS * 16);
+        maxpool_bwd_kernel<<<blocks, 256, 0, st>>>(x, dy, dx, N, H, W, C, OH, OW, py, px);
+        PXL_CHECK_LAUNCH();
+    }
     return 0;
 }
 

@@ -90,8 +90,8 @@ __device__ __forceinline__ void y_support(int i, int h, int H, float sh, bool ac
 //   * the ~2/sh contributing high-res rows are staged G at a time by the whole CTA (coalesced loads,
 //     G*W/128 independent loads per thread), stored at x + x/R so that lanes walking supports that
 //     start R apart hit distinct banks;
-//   * work item = (staged row g, column j): a SUP-long dot product from shared memory, one shared
-//     atomicAdd per item.
+//   * thread = column j: SUP-long dot products from shared memory over the staged rows in order, so the
+//     result does not depend on thread timing.
 template <bool NHWC>
 __global__ void __launch_bounds__(128)
 bilinear_bwd_kernel(const float* __restrict__ gout, float* __restrict__ gin, int C, int h, int w, int H, int W,
@@ -163,28 +163,31 @@ bilinear_bwd_kernel(const float* __restrict__ gout, float* __restrict__ gin, int
             }
         }
         __syncthreads();
-        for (int item = threadIdx.x; item < rows * w; item += blockDim.x) {
-            const int g = item / w, j = item - g * w;
-            const int y = y0g + g;
-            const float fy = src_index(sh, y, ac);
-            const int yy0 = (int)fy;
-            const int yy1 = yy0 + (yy0 < h - 1 ? 1 : 0);
-            const float ly1 = fy - (float)yy0;
-            float wy = 0.f;
-            if (yy0 == i) wy += 1.f - ly1;
-            if (yy1 == i) wy += ly1;
-            if (wy == 0.f) continue;
+        for (int j = threadIdx.x; j < w; j += blockDim.x) {
             const int4 m = meta[j];
             const float* wt = wtab + j * SUP;
-            const float* rp = rb + g * rowbuf;
-            int pidx = m.z, rem = m.w;
-            float sacc = 0.f;
-            for (int t = 0; t < m.y; ++t) {
-                sacc = fmaf(rp[pidx], wt[t], sacc);
-                ++pidx;
-                if (++rem == R) { rem = 0; ++pidx; }
+            float a = acc[j];
+            for (int g = 0; g < rows; ++g) {             // rows in order: the sum does not depend on thread timing
+                const int y = y0g + g;
+                const float fy = src_index(sh, y, ac);
+                const int yy0 = (int)fy;
+                const int yy1 = yy0 + (yy0 < h - 1 ? 1 : 0);
+                const float ly1 = fy - (float)yy0;
+                float wy = 0.f;
+                if (yy0 == i) wy += 1.f - ly1;
+                if (yy1 == i) wy += ly1;
+                if (wy == 0.f) continue;
+                const float* rp = rb + g * rowbuf;
+                int pidx = m.z, rem = m.w;
+                float sacc = 0.f;
+                for (int t = 0; t < m.y; ++t) {
+                    sacc = fmaf(rp[pidx], wt[t], sacc);
+                    ++pidx;
+                    if (++rem == R) { rem = 0; ++pidx; }
+                }
+                a += sacc * wy;
             }
-            atomicAdd(acc + j, sacc * wy);
+            acc[j] = a;
         }
     }
     __syncthreads();

@@ -34,7 +34,7 @@ class Conv2d(nn.Module):
     def forward(self, x):
         w = self.weight
         if x.shape[1] > self.in_channels:
-            # input lanes were zero-padded (e.g. 21 -> 32 so the tcgen05 kernel applies): pad the weight
+            # input lanes were zero-padded (e.g. 21 -> 32 so the wgmma kernel applies): pad the weight
             # with matching zero channels; tiny tensor, plain autograd ops
             w = torch.nn.functional.pad(w, (0, 0, 0, 0, 0, x.shape[1] - self.in_channels)).contiguous(memory_format=CL)
         return ops.conv2d(ops.as_cl(x), w, self.bias, self.stride, self.padding, self.dilation, self.out_lanes,

@@ -16,15 +16,15 @@ from . import _lib
 from ._lib import ConvGeom, ConvTcExt, call
 
 CL = torch.channels_last
-# conv precision policy (pxl_conv_geom.precision): 0 fp32 FFMA, 1 TF32 tcgen05, 2 3xTF32 tcgen05,
-# 3 fp16-pair x3 tcgen05 (fp32-grade), 4 single fp16 tcgen05 (TF32-grade)
+# conv precision policy (pxl_conv_geom.precision): 0 fp32 FFMA, 1 TF32 wgmma, 2 3xTF32 wgmma,
+# 3 fp16-pair x3 wgmma (fp32-grade), 4 single fp16 wgmma (TF32-grade)
 PRECISION = {'fp32': 0, 'tf32': 1, 'tf32x3': 2, 'f16x3': 3, 'f16': 4}
-H16_FALLBACK = {3: 2, 4: 1}     # shapes the kind::f16 kernels do not cover run on the tf32 kernels of the same grade
+H16_FALLBACK = {3: 2, 4: 1}     # shapes the f16 wgmma kernels do not cover run on the tf32 kernels of the same grade
 H16_ACT_SCALE = 16.0            # fixed power-of-two scales of fp16 pairs (csrc/h16_prep.cu): activations saturate
 H16_W_SCALE = 256.0             # beyond +-4094, weights beyond +-255 (counted: h16_status())
 H16_GRAD_TARGET_LOG2 = 14       # gradients: per-tensor scale putting the absmax in (2^13, 2^14]
 _conv_precision = 0
-_WGRAD_TC_STRIDES = (1, 2)      # convolution strides the tcgen05 wgrad kernel handles
+_WGRAD_TC_STRIDES = (1, 2)      # convolution strides the wgmma wgrad kernel handles
 
 
 def set_conv_precision(name):
@@ -529,7 +529,7 @@ def h16_supported(Cin, mul, div):
 
 
 def tc_supported(Cin, mul, div):
-    """Shapes covered by the tcgen05 forward/dgrad kernel (csrc/conv_tc.cu): stride 1 and 2 forward
+    """Shapes covered by the wgmma forward/dgrad kernel (csrc/conv_tc.cu): stride 1 and 2 forward
     (mul), and the dgrad of a stride-2 convolution (div == 2, decomposed by output parity)."""
     return Cin % 32 == 0 and ((div == 1 and mul in (1, 2)) or (div == 2 and mul == 1))
 
@@ -560,7 +560,7 @@ def _tc_launch(geom, taps, ext, x_parts, w_parts, bias, out):
 def conv_raw(x, w_packed, bias, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div, out=None, precision=None, bn_stats=None,
              accumulate=False):
     """Launch the NHWC tap-table convolution on raw buffers.  w_packed: [Cout][ntaps][Cin] contiguous.
-    precision 0: FFMA kernel; 1: tcgen05 single-pass TF32; 2: tcgen05 3xTF32 (operands split on the
+    precision 0: FFMA kernel; 1: wgmma single-pass TF32; 2: wgmma 3xTF32 (operands split on the
     fly).  Shapes the tensor-core kernel does not cover (Cin % 32 != 0, other strides) use the FFMA kernel."""
     ntaps = len(taps) // 2
     prec = _conv_precision if precision is None else precision
@@ -571,7 +571,7 @@ def conv_raw(x, w_packed, bias, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div,
             out.zero_()
     if prec >= 3 and not h16_supported(Cin, mul, div):
         if isinstance(x, H16) or isinstance(w_packed, H16):
-            raise ValueError('fp16-pair operands given for a shape the kind::f16 kernel does not cover')
+            raise ValueError('fp16-pair operands given for a shape the f16 wgmma kernel does not cover')
         prec = H16_FALLBACK[prec]
     if prec >= 3:
         want_lo = prec == 3
@@ -648,7 +648,7 @@ def conv_raw(x, w_packed, bias, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div,
 
 
 def conv_tc_status():
-    """0 when every tcgen05 pipeline so far completed; otherwise the role whose mbarrier wait timed out."""
+    """0 when every wgmma pipeline so far completed; otherwise the role whose mbarrier wait timed out."""
     return int(_lib.load().pxl_conv_tc_status())
 
 
@@ -658,7 +658,7 @@ def conv_wgrad_raw(x, dy, dw, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div, p
     prec = _conv_precision if precision is None else precision
     if prec >= 3 and not (div == 1 and mul in _WGRAD_TC_STRIDES and Cin % 64 == 0 and ldo % 64 == 0):
         if isinstance(x, H16) or isinstance(dy, H16):
-            raise ValueError('fp16-pair operands given for a shape the kind::f16 wgrad kernel does not cover')
+            raise ValueError('fp16-pair operands given for a shape the f16 wgmma wgrad kernel does not cover')
         prec = H16_FALLBACK[prec]
     if prec >= 3:
         want_lo = prec == 3
@@ -965,7 +965,7 @@ class _Stem(torch.autograd.Function):
 
     fp32 mode: the dedicated FFMA kernels.  Tensor-core modes: the image is unfolded once into a
     [pixels, 160] matrix (147 taps*channels + 13 zero lanes) and the stem runs as a flat 1x1 convolution on
-    tcgen05, forward and wgrad sharing the matrix (19.9 GFLOP each on the 513x513 x16 batch)."""
+    wgmma, forward and wgrad sharing the matrix (19.9 GFLOP each on the 513x513 x16 batch)."""
 
     @staticmethod
     def forward(ctx, img, weight, sums):
@@ -1181,9 +1181,9 @@ def bn_act(x, gamma, beta, running_mean, running_var, training=True, momentum=0.
 
 # Weight gradients are off the critical path of the backward pass (nothing reads them before the optimiser step), so
 # they could run on a side stream right after the dX pair they consume exists, overlapping the HBM-bound BatchNorm
-# backward launches.  NEGATIVE RESULT (measured, B200, MT step): 53.8 ms -> 76.4 ms.  The wgrad CTAs (200 KB of
-# shared memory each) take SMs away from the persistent one-CTA-per-SM convolutions of the critical path, which then
-# wait for them - a priority inversion the default stream cannot be prioritised out of.  Opt-in: PXL_WGRAD_SIDE_STREAM=1.
+# backward launches.  Off by default: the wgrad CTAs (up to ~220 KB of shared memory each) take SMs away from the
+# persistent one-CTA-per-SM convolutions of the critical path, which then wait for them.  Not measured on the H100.
+# Opt-in: PXL_WGRAD_SIDE_STREAM=1.
 # block outputs: ReLU mask for the backward as 1 byte per 4 values (A/B switch; 0 re-reads the fp32 result)
 BN_RELU_MASK = _os.environ.get('PXL_BN_RELU_MASK', '1') != '0'
 WGRAD_SIDE_STREAM = _os.environ.get('PXL_WGRAD_SIDE_STREAM', '0') != '0'
@@ -1242,7 +1242,7 @@ def is_carrier(t):
 
 class _ConvBnAct(torch.autograd.Function):
     """Bottleneck building block (resnet.py:33-48): bias-free conv -> train-mode (Sync)BN (batchnorm.py:48-78)
-    -> (+ residual) -> (ReLU), ONE autograd node on the kind::f16 tensor-core path.
+    -> (+ residual) -> (ReLU), ONE autograd node on the f16 wgmma tensor-core path.
 
     Forward: the convolution reads the fp16 pair of its input, its epilogue produces the BN statistics, and the BN
     apply launch writes its result directly as the fp16 pair of the next convolution (``out_mode`` 'pair': only the

@@ -12,7 +12,7 @@ from .utils import cmd, logger
 
 
 def create_parser(algorithm):
-    parser = argparse.ArgumentParser(description='PixelSSL-B200 Static Script Parser')
+    parser = argparse.ArgumentParser(description='PixelSSL-H100 Static Script Parser')
     if algorithm not in ssl_algorithm.SSL_ALGORITHMS:
         logger.log_err('Unknown semi-supervised learning algorithm: {0}\n'
                        'The support algorithms are: {1}\n'.format(algorithm, ssl_algorithm.SSL_ALGORITHMS))

@@ -1,4 +1,4 @@
-"""Adversarial SSL (pixelssl/ssl_algorithm/ssl_adv.py:118-283) on the B200 kernels.
+"""Adversarial SSL (pixelssl/ssl_algorithm/ssl_adv.py:118-283) on the H100 kernels.
 
 step 1 (task model): forward -> softmax -> FC discriminator (frozen for this step) -> CE on the
 labeled rows + BCE(confidence, real) adversarial terms -> backward -> SGD.

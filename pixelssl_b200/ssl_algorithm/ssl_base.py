@@ -115,8 +115,8 @@ def device_prefetch(data_loader):
             yield batch
         return
     # the copy stream, the staging slots and their "consumed" events live as long as the process: a new side stream per
-    # epoch gets no cached blocks from torch's (per-stream) allocator pools, and the cudaMalloc of the 67 MB slots
-    # cost ~130 ms at the start of three epochs out of four (tools/e2e_probe2.py)
+    # epoch gets no cached blocks from torch's (per-stream) allocator pools, and a cudaMalloc of the 67 MB slots at the
+    # start of an epoch stalls the step (tools/e2e_probe2.py)
     state = _prefetch_state.get(torch.cuda.current_device())
     if state is None:
         state = _prefetch_state[torch.cuda.current_device()] = {

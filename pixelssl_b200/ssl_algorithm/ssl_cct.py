@@ -1,4 +1,4 @@
-"""Cross-Consistency Training (pixelssl/ssl_algorithm/ssl_cct.py:226-301, 438-745) on the B200 kernels.
+"""Cross-Consistency Training (pixelssl/ssl_algorithm/ssl_cct.py:226-301, 438-745) on the H100 kernels.
 
 One shared encoder (the task model) and K perturbation decoders (VAT, Dropout, G-Cutout, context /
 object masking, feature drop, feature noise).  Per step: labeled rows -> task model -> CE; unlabeled

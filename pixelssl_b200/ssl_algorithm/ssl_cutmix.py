@@ -1,4 +1,4 @@
-"""CutMix consistency (pixelssl/ssl_algorithm/ssl_cutmix.py:132-255) on the B200 kernels.
+"""CutMix consistency (pixelssl/ssl_algorithm/ssl_cutmix.py:132-255) on the H100 kernels.
 
 Per step: host box masks (numpy RNG, identical draws to the reference) -> bit-exact device mix
 of the two unlabeled halves -> student fwd on the labeled rows + CE -> teacher fwd (no grad) on

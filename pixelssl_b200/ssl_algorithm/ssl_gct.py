@@ -1,4 +1,4 @@
-"""Guided Collaborative Training (pixelssl/ssl_algorithm/ssl_gct.py:176-298, 401-480) on the B200 kernels.
+"""Guided Collaborative Training (pixelssl/ssl_algorithm/ssl_gct.py:176-298, 401-480) on the H100 kernels.
 
 Per step: (0) no-grad forwards of the two task models; flaw detector (FD) on both (graph kept for
 step 2); handled flaw maps (clamp -> separable Gaussian blur -> clip -> min-max) and the dynamic-

@@ -1,4 +1,4 @@
-"""Pixel-wise Mean Teacher on the B200 kernels: the per-step loop of
+"""Pixel-wise Mean Teacher on the H100 kernels: the per-step loop of
 pixelssl/ssl_algorithm/ssl_mt.py:124-224 with the same order of operations
 
     zero_grad -> student fwd -> CE(labeled) -> teacher fwd (no grad) + teacher CE (meter only)

@@ -1,4 +1,4 @@
-"""SSL_S4L on the B200 kernels: plugin mirror of pixelssl/ssl_algorithm/ssl_s4l.py (rotation-based
+"""SSL_S4L on the H100 kernels: plugin mirror of pixelssl/ssl_algorithm/ssl_s4l.py (rotation-based
 self-supervised semi-supervised learning): same parser arguments, export function, ``_SSLBase`` methods, meter
 names and checkpoint layout.
 

@@ -1,4 +1,4 @@
-"""DeepLab-v2 head on the B200 kernels (task/sseg/module/deeplab_v2.py:13-85): backbone ->
+"""DeepLab-v2 head on the H100 kernels (task/sseg/module/deeplab_v2.py:13-85): backbone ->
 ASPP (4 dilated 3x3 convs 2048->C summed, ONE 36-tap kernel here) -> bilinear upsample
 (align_corners=True) to the input size."""
 import torch.nn as nn

@@ -1,4 +1,4 @@
-"""PSPNet on the B200 kernels: module tree and forward order of task/sseg/module/_pspnet.py:57-128
+"""PSPNet on the H100 kernels: module tree and forward order of task/sseg/module/_pspnet.py:57-128
 (pyramid pooling bins 1/2/3/6 -> 1x1 conv + BN + ReLU -> bilinear (align_corners=False) -> concat with
 the backbone features -> 3x3 conv 4096->512 + BN + ReLU -> conv1x1 + 3 x PixelShuffle decoder ->
 bilinear (align_corners=True) to the input size)."""

@@ -1,4 +1,4 @@
-"""Dilated ResNet backbone on the B200 kernels: parameter tree and forward order of
+"""Dilated ResNet backbone on the H100 kernels: parameter tree and forward order of
 task/sseg/module/backbone/resnet.py:13-131 (Bottleneck, strides/dilations per output stride,
 multi-grid layer4), with BN+ReLU(+residual) fused and NHWC activations throughout."""
 import math

@@ -10,12 +10,12 @@ if ROOT not in sys.path:
 GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 # Convolution precision modes every whole-network / whole-step GPU golden is run under (fixture params, so the
-# mode shows up in the test id): the exact-fp32 FFMA kernels and the fp32-grade tcgen05 modes that bench.py times.
+# mode shows up in the test id): the exact-fp32 FFMA kernels and the fp32-grade wgmma modes that bench.py times.
 TEST_PRECISIONS = [p for p in os.environ.get('PXL_TEST_PRECISIONS', 'fp32,tf32x3,f16x3').split(',') if p]
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100; run with -m gpu)')
     config.addinivalue_line('markers', 'slow: CPU test that takes more than a few seconds')
 
 

@@ -20,7 +20,7 @@ CL = torch.channels_last
 @pytest.fixture(scope='module', params=TEST_PRECISIONS)
 def ops(request):
     """Every test of this module runs once per convolution precision mode (tests/conftest.py): the exact FFMA
-    path and the tcgen05 paths bench.py measures are held to the same goldens."""
+    path and the wgmma paths bench.py measures are held to the same goldens."""
     if not torch.cuda.is_available():
         pytest.skip('needs a GPU')
     from pixelssl_b200 import ops as _ops

@@ -22,7 +22,7 @@ CL = torch.channels_last
 @pytest.fixture(scope='module', params=TEST_PRECISIONS)
 def ops(request):
     """Every test of this module runs once per convolution precision mode (tests/conftest.py): the exact FFMA
-    path and the tcgen05 paths bench.py measures are held to the same goldens."""
+    path and the wgmma paths bench.py measures are held to the same goldens."""
     if not torch.cuda.is_available():
         pytest.skip('needs a GPU')
     from pixelssl_b200 import ops as _ops
@@ -110,8 +110,8 @@ def test_auxiliary_decoder_matches_oracle(ops, kind):
     tol = 5e-3 if kind == 'vat' else 2e-5             # VAT: direction of a normalised gradient (amplifies round-off)
     # The decoders are ReLU networks: an activation within round-off of zero takes either branch, and ONE such flip
     # moves isolated gradient entries by percents of the maximum (measured: the same single element, 3e-2, in the cut /
-    # context / fd cases whenever the accumulation order of the first convolution changes, e.g. with
-    # PXL_TC_NACC_F16X3=2; VAT's normalised adversarial direction flips a few more).  So gradients are compared on all
+    # context / fd cases whenever the accumulation order of the first convolution changes; VAT's normalised
+    # adversarial direction flips a few more).  So gradients are compared on all
     # but the worst 0.2 % of the entries (1 % for VAT) and the outputs, which are continuous, on every entry.
     cmp = (lambda a, b: rel_q(a, b, 1e-2)) if kind == 'vat' else rel_q
     e_out, e_in = rel(out[:, :nc], ref), cmp(xg.grad, xc.grad)

@@ -1,10 +1,8 @@
-"""tcgen05 convolution (csrc/conv_tc.cu) against the FFMA fp32 kernel and the torch-CPU oracle op.
+"""wgmma convolution (csrc/conv_tc.cu) against the FFMA fp32 kernel and the torch-CPU oracle op.
 
-precision 2 (3xTF32: hi/lo operand split, fp32 TMEM accumulation) must agree with fp32 to 5e-5
-relative (measured 5e-7 at K=64 .. 2e-5 at K=2304: the tensor core's fp32 accumulator is not an
-IEEE round-to-nearest adder, so the error grows ~sqrt(K)); precision 1 (single TF32 pass, what cuDNN does by default for the reference on GPU) to
-2e-3.  The mbarrier watchdog must stay silent."""
-import os
+precision 2 (3xTF32: hi/lo operand split, fp32 accumulation) must agree with fp32 to 5e-5 relative (the
+tensor core's fp32 accumulator is not an IEEE round-to-nearest adder, so the error grows with K); precision 1
+(single TF32 pass, what cuDNN does by default for the reference on GPU) to 2e-3.  The mbarrier watchdog must stay silent."""
 
 import pytest
 import torch
@@ -184,7 +182,7 @@ def test_h16_pair_split_is_exact_to_22_bits(ops):
 
 
 def test_tf32_operand_rounding_probe(ops):
-    """Documents what kind::tf32 does with the low 13 mantissa bits of raw fp32 operands."""
+    """Documents what tf32 wgmma does with the low 13 mantissa bits of raw fp32 operands."""
     x = torch.full((1, 32, 8, 16), 1.0 + 2.0 ** -11 + 2.0 ** -12).cuda().contiguous(memory_format=CL)   # low bits set
     w = torch.zeros(32, 32, 1, 1).cuda().contiguous(memory_format=CL)
     w[0, 0] = 1.0
@@ -221,24 +219,10 @@ def test_bn_statistics_fused_in_epilogue(ops, shape, precision):
     assert rel(a, b) <= 1e-5
 
 
-def test_cta_pair_kernel_opt_in_subprocess():
-    """The cta_group::2 (CTA-pair) variant is opt-in (PXL_TC_PAIR=1, read once per process): run a few of the
-    parity cases of this file in a child process with it enabled so the path stays verified."""
-    import subprocess
-    import sys
-    env = dict(os.environ, PXL_TC_PAIR='1')
-    here = os.path.abspath(__file__)
-    r = subprocess.run([sys.executable, '-m', 'pytest', here, '-q', '-x', '-m', 'gpu', '-k',
-                        'not subprocess and (forward_and_dgrad or fused or aspp)'],
-                       env=env, capture_output=True, text=True, timeout=600,
-                       cwd=os.path.dirname(os.path.dirname(here)))
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-
-
 @pytest.mark.parametrize('precision,tol_y,tol_w', [('tf32x3', 2e-5, 5e-5), ('tf32', 3e-3, 3e-3), ('f16x3', 2e-5, 5e-5), ('f16', 3e-3, 3e-3)])
 @pytest.mark.parametrize('N,H,W', [(2, 65, 65), (1, 97, 129), (2, 40, 36)])
 def test_stem_tensor_core_path(ops, N, H, W, precision, tol_y, tol_w):
-    """7x7/2 stem as im2col (pxl_stem_im2col) + flat 1x1 tcgen05 convolution, forward, weight gradient and the
+    """7x7/2 stem as im2col (pxl_stem_im2col) + flat 1x1 wgmma convolution, forward, weight gradient and the
     fused BatchNorm sums, against torch CPU fp32 (resnet.py:69,121)."""
     gs = torch.Generator().manual_seed(H * 7 + W)
     img = torch.randn(N, 3, H, W, generator=gs)

@@ -1,4 +1,4 @@
-"""BASELINE.json's configurations at their FULL sizes on the tcgen05 path bench.py measures (fp16-pair x3): every algorithm must step with
+"""BASELINE.json's configurations at their FULL sizes on the wgmma path bench.py measures (fp16-pair x3): every algorithm must step with
 finite losses and a silent pipeline watchdog, and the size-independent properties of the hot kernels must hold on
 full-size tensors (the oracle cannot run these sizes in seconds; small-size parity is in the other test files).
 

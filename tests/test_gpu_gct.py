@@ -20,7 +20,7 @@ CL = torch.channels_last
 @pytest.fixture(scope='module', params=TEST_PRECISIONS)
 def ops(request):
     """Every test of this module runs once per convolution precision mode (tests/conftest.py): the exact FFMA
-    path and the tcgen05 paths bench.py measures are held to the same goldens."""
+    path and the wgmma paths bench.py measures are held to the same goldens."""
     if not torch.cuda.is_available():
         pytest.skip('needs a GPU')
     from pixelssl_b200 import ops as _ops
@@ -110,7 +110,7 @@ def test_flaw_detector_forward_backward(ops):
     # The 99.8 % quantile of the input-gradient error counts LeakyReLU kink flips: the CPU oracle's own fp32
     # evaluation is 4.6e-4 (max 1.1e-3) away from its fp64 evaluation, and a 1e-5 relative input perturbation moves it
     # by the same amount (measured, oracle/gct_oracle.py).  The exact-fp32 FFMA path stays at the 2e-3 it was written
-    # for; the tensor-core modes carry ~2e-5 forward error on these K = 4x4x512 reductions (fp32 TMEM accumulation
+    # for; the tensor-core modes carry ~2e-5 forward error on these K = 4x4x512 reductions (truncating fp32 tensor-core accumulation
     # truncates, see tests/test_gpu_conv_tc.py) and flip a few more kinks: 2e-2 on the quantile, median still tight.
     med = float(((pg.grad.cpu().double() - pc.grad.double()).abs() / pc.grad.double().abs().max()).median())
     assert e_out <= 1e-4 and e_in <= (2e-3 if ops.get_conv_precision() == 0 else 2e-2) and med <= 2e-4, (e_out, e_in, med)

@@ -29,7 +29,7 @@ G = os.path.join(os.path.dirname(__file__), 'golden')
 @pytest.fixture(scope='module', params=TEST_PRECISIONS)
 def eng(request):
     """Every whole-network / whole-step golden runs once per convolution precision mode (tests/conftest.py):
-    the exact FFMA path AND the tcgen05 paths that bench.py measures are held to the same reference vectors."""
+    the exact FFMA path AND the wgmma paths that bench.py measures are held to the same reference vectors."""
     if not torch.cuda.is_available():
         pytest.skip('needs a GPU')
     import pixelssl_b200

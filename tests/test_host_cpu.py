@@ -114,34 +114,42 @@ def test_param_arena_layout_and_segments():
     assert sum(b - a for s in segs for a, b in s) == arena.numel
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference tree only exists in the build container')
-def test_register_into_unmodified_pixelssl():
+def _host_ref():
+    """tests/golden/host_reference.json.gz: the reference's own answers to the questions below (oracle/make_golden.py host)"""
+    import gzip
+    import json
+    with gzip.open(os.path.join(G, 'host_reference.json.gz'), 'rt') as f:
+        return json.load(f)
+
+
+def _parser_table(parser, with_options=True):
+    from oracle.make_golden import parser_table
+    return parser_table(parser, with_options)
+
+
+def test_register_into_pixelssl_layout():
+    """register_into_pixelssl on a package laid out like PixelSSL (pixelssl.ssl_algorithm, pixelssl.nn.data): every
+    algorithm module is replaced, and the sampler the proxy looks up yields the reference sampler's stream."""
     import sys
-    sys.path.insert(0, '/root/reference')
-    import pixelssl
+    import types
     import pixelssl_b200
-    pixelssl_b200.register_into_pixelssl(pixelssl)
+    pkg = types.ModuleType('pixelssl')
+    pkg.ssl_algorithm = types.ModuleType('pixelssl.ssl_algorithm')
+    pkg.ssl_algorithm.SSL_ALGORITHMS = list(_host_ref()['ssl_algorithms'])
+    pkg.nn = types.ModuleType('pixelssl.nn')
+    pkg.nn.data = types.ModuleType('pixelssl.nn.data')
+    pixelssl_b200.register_into_pixelssl(pkg)
+    assert sorted(pixelssl_b200.SSL_ALGORITHMS) == sorted(pkg.ssl_algorithm.SSL_ALGORITHMS)
     for name in pixelssl_b200.SSL_ALGORITHMS:
-        mod = pixelssl.ssl_algorithm.__dict__[name]
+        mod = pkg.ssl_algorithm.__dict__[name]
         assert mod.__name__.startswith('pixelssl_b200.')
         assert callable(getattr(mod, name)) and callable(mod.add_parser_arguments)
-        assert name in pixelssl.ssl_algorithm.SSL_ALGORITHMS
-    # the proxy's sampler lookup (pixelssl.nn.data.TwoStreamBatchSampler) now resolves to the rank-aware one,
-    # which at world size 1 yields exactly what the reference's own class yields
-    from pixelssl.nn import data as nndata
-    import importlib
-    assert nndata.TwoStreamBatchSampler.__module__ == 'pixelssl_b200.nn.data'
-    ref_cls = importlib.reload(importlib.import_module('pixelssl.nn.data')).TwoStreamBatchSampler
+    assert pkg.nn.data.TwoStreamBatchSampler.__module__ == 'pixelssl_b200.nn.data'
     np.random.seed(5)
-    want = [list(map(int, b)) for b in ref_cls(list(range(9)), list(range(50, 83)), 2, 3)]
-    pixelssl_b200.register_into_pixelssl(pixelssl)
-    np.random.seed(5)
-    got = [list(map(int, b)) for b in nndata.TwoStreamBatchSampler(list(range(9)), list(range(50, 83)), 2, 3)]
-    assert got == want and len(got) == 11
-    # the reference's own parser builder accepts the engine's algorithm modules
-    from pixelssl import runner
-    parser = runner.create_parser('ssl_mt')
-    ns = parser.parse_args(['--cons-scale', '1.0', '--ema-decay', '0.99'])
+    got = [list(map(int, b)) for b in pkg.nn.data.TwoStreamBatchSampler(list(range(9)), list(range(50, 83)), 2, 3)]
+    assert got == _host_ref()['sampler_seed5'] and len(got) == 11
+    from pixelssl_b200 import runner
+    ns = runner.create_parser('ssl_mt').parse_args(['--cons-scale', '1.0', '--ema-decay', '0.99'])
     assert ns.cons_scale == 1.0 and ns.ema_decay == 0.99
 
 
@@ -225,138 +233,83 @@ def test_deferred_step_log_prints_same_text_one_interval_late(monkeypatch):
     assert len(emitted) == 3
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference tree only exists in the build container')
 @pytest.mark.parametrize('name,backbone', [('deeplabv2', 'resnet101'), ('pspnet', 'resnet50'), ('pspnet', 'resnet101')])
 def test_task_model_state_dict_and_param_groups_match_reference(name, backbone):
     """Checkpoint compatibility (SURVEY 8f rank 3): same state_dict keys, shapes and dtypes as the reference task
     model (so its .ckpt files load), same LR groups in the same order (task/sseg/model.py:45-48,103-107)."""
-    import sys
     import torch.utils.model_zoo as mz
-    saved = (mz.load_url, torch.nn.Module.cuda, torch.Tensor.cuda)
+    saved = mz.load_url
     mz.load_url = lambda *a, **k: {}
-    for p in ('/root/reference', '/root/reference/task/sseg'):
-        if p not in sys.path:
-            sys.path.insert(0, p)
     try:
-        import model as ref_model                        # task/sseg/model.py of the reference
         from pixelssl_b200 import runner
         from pixelssl_b200.task.sseg import model as eng_model
         args = runner.build_args({'ssl_algorithm': 'ssl_null', 'lr': 0.00025, 'momentum': 0.9, 'weight_decay': 0.0005,
                                   'epochs': 2, 'batch_size': 2, 'unlabeled_batch_size': 0, 'ignore_unlabeled': True,
                                   'backbone': backbone}, iters_per_epoch=5)
-        ref = getattr(ref_model, name)()(args)
         eng = getattr(eng_model, name)()(args)
-        rs, es = ref.state_dict(), eng.state_dict()
-        assert list(rs.keys()) == list(es.keys())
-        for k in rs:
-            assert tuple(rs[k].shape) == tuple(es[k].shape) and rs[k].dtype == es[k].dtype, k
-        rid = {id(p): n for n, p in ref.named_parameters()}
-        eid = {id(p): n for n, p in eng.named_parameters()}
-        assert len(ref.param_groups) == len(eng.param_groups)
-        for rg, eg in zip(ref.param_groups, eng.param_groups):
-            assert rg['lr'] == eg['lr']
-            assert [rid[id(p)] for p in rg['params']] == [eid[id(p)] for p in eg['params']]
     finally:
-        mz.load_url, torch.nn.Module.cuda, torch.Tensor.cuda = saved
+        mz.load_url = saved
+    ref = _host_ref()['models']['%s-%s' % (name, backbone)]
+    assert [[k, list(v.shape), str(v.dtype)] for k, v in eng.state_dict().items()] == ref['state']
+    eid = {id(p): n for n, p in eng.named_parameters()}
+    assert [[g['lr'], [eid[id(p)] for p in g['params']]] for g in eng.param_groups] == ref['param_groups']
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference tree only exists in the build container')
 @pytest.mark.parametrize('alg', ['ssl_null', 'ssl_mt', 'ssl_cutmix', 'ssl_adv', 'ssl_gct', 'ssl_cct'])
 def test_checkpoint_dict_keys_match_reference(alg):
     """Every algorithm saves the same top-level checkpoint keys as the reference's ``_save_checkpoint``
     (e.g. ssl_mt.py:296-307), so checkpoints are interchangeable between the two."""
-    def keys_of(path):
-        src = open(path).read()
-        body = src[src.index('def _save_checkpoint'):]
-        body = body[body.index('state = {'):]
-        body = body[:body.index('}') + 1]
-        return sorted(set(re.findall(r"'([a-z_]+)'\s*:", body)))
-    ref = keys_of('/root/reference/pixelssl/ssl_algorithm/%s.py' % alg)
-    eng = keys_of(os.path.join(ROOT, 'pixelssl_b200', 'ssl_algorithm', '%s.py' % alg))
-    assert ref == eng and 'algorithm' in eng and 'epoch' in eng
+    src = open(os.path.join(ROOT, 'pixelssl_b200', 'ssl_algorithm', '%s.py' % alg)).read()
+    body = src[src.index('def _save_checkpoint'):]
+    body = body[body.index('state = {'):]
+    body = body[:body.index('}') + 1]
+    eng = sorted(set(re.findall(r"'([a-z_]+)'\s*:", body)))
+    assert _host_ref()['checkpoint_keys'][alg] == eng and 'algorithm' in eng and 'epoch' in eng
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference tree only exists in the build container')
 @pytest.mark.parametrize('alg', ['ssl_null', 'ssl_mt', 'ssl_cutmix', 'ssl_adv', 'ssl_gct', 'ssl_cct'])
 def test_algorithm_parser_arguments_match_reference(alg):
     """add_parser_arguments of every algorithm module: same options, defaults, types and choices as the
     reference's (e.g. ssl_mt.py:27-38), so its scripts/configs parse identically."""
     import argparse
-    import importlib
-    import sys
-    if '/root/reference' not in sys.path:
-        sys.path.insert(0, '/root/reference')
-    ref_mod = importlib.import_module('pixelssl.ssl_algorithm.' + alg)
-    if not ref_mod.__name__.startswith('pixelssl.') or 'pixelssl_b200' in getattr(ref_mod, '__file__', ''):
-        ref_mod = importlib.reload(ref_mod)
     from pixelssl_b200 import ssl_algorithm as eng
-    pr, pe = argparse.ArgumentParser(), argparse.ArgumentParser()
-    ref_mod.add_parser_arguments(pr)
+    pe = argparse.ArgumentParser()
     getattr(eng, alg).add_parser_arguments(pe)
-
-    def table(parser):
-        return {a.dest: (a.default, getattr(a.type, '__name__', a.type), a.choices, tuple(a.option_strings))
-                for a in parser._actions if a.dest != 'help'}
-    assert table(pr) == table(pe)
+    assert _host_ref()['alg_parser'][alg] == _parser_table(pe)
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference tree only exists in the build container')
 def test_full_argument_set_matches_reference_runner_and_sseg_proxy():
     """runner.create_parser + the proxy/task arguments: every option the reference's ``pixelssl.runner.create_parser``
     + ``task/sseg/proxy.add_parser_arguments`` defines exists here with the same default and type."""
-    import sys
-    for p in ('/root/reference', '/root/reference/task/sseg'):
-        if p not in sys.path:
-            sys.path.insert(0, p)
-    import importlib
-    rr = importlib.import_module('pixelssl.runner')
-    # the algorithm table may have been swapped by an earlier register_into_pixelssl test: compare with ssl_null,
-    # whose options both implementations define identically (tested above)
-    sp = importlib.import_module('proxy')
     from pixelssl_b200 import runner as er
-    pr = rr.create_parser('ssl_null')
-    sp.add_parser_arguments(pr)
     pe = er.create_parser('ssl_null')
     er.add_proxy_arguments(pe)
-
-    def table(parser):
-        return {a.dest: (a.default, getattr(a.type, '__name__', a.type), a.choices) for a in parser._actions if a.dest != 'help'}
-    te = table(pe)
+    te = _parser_table(pe, with_options=False)
     # engine-only option: the reference hard-codes the pretrained-backbone URL per backbone (task/sseg/model.py:69-80);
     # the engine exposes the same choice as a flag whose default 'auto' resolves to exactly those URLs
-    assert te.pop('pretrained_backbone') == ('auto', 'str', None)
-    assert table(pr) == te
+    assert te.pop('pretrained_backbone') == ['auto', 'str', None]
+    assert _host_ref()['full_parser'] == te
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference tree only exists in the build container')
 @pytest.mark.parametrize('name', ['steplr', 'multisteplr', 'exponentiallr', 'cosineannealinglr', 'polynomiallr'])
 def test_lr_scheduler_wrappers_follow_the_reference(name):
     """Every lrer export yields the reference's learning-rate trajectory (pixelssl/nn/lrer.py:51-179) on a toy
     two-group optimizer, including the per-scheduler defaults behind the parser's -1 placeholders."""
     import argparse
-    import importlib
-    import sys
-    if '/root/reference' not in sys.path:
-        sys.path.insert(0, '/root/reference')
-    ref = importlib.import_module('pixelssl.nn.lrer')
     from pixelssl_b200.nn import lrer as eng
-
-    def run(mod):
-        parser = argparse.ArgumentParser()
-        mod.add_parser_arguments(parser)
-        args = parser.parse_args([])
-        args.epochs, args.iters_per_epoch = 6, 4
-        w = [torch.nn.Parameter(torch.zeros(2)), torch.nn.Parameter(torch.zeros(2))]
-        opt = torch.optim.SGD([{'params': [w[0]], 'lr': 0.1}, {'params': [w[1]], 'lr': 1.0}], lr=0.1, momentum=0.9)
-        sched = getattr(mod, name)(args)(opt)
-        traj = []
-        steps = args.epochs * args.iters_per_epoch - 1 if name == 'polynomiallr' else args.epochs
-        for _ in range(steps):
-            traj.append([g['lr'] for g in opt.param_groups])
-            opt.step()
-            sched.step()
-        return traj
-    np.testing.assert_allclose(run(eng), run(ref), rtol=1e-12)
+    parser = argparse.ArgumentParser()
+    eng.add_parser_arguments(parser)
+    args = parser.parse_args([])
+    args.epochs, args.iters_per_epoch = 6, 4
+    w = [torch.nn.Parameter(torch.zeros(2)), torch.nn.Parameter(torch.zeros(2))]
+    opt = torch.optim.SGD([{'params': [w[0]], 'lr': 0.1}, {'params': [w[1]], 'lr': 1.0}], lr=0.1, momentum=0.9)
+    sched = getattr(eng, name)(args)(opt)
+    traj = []
+    for _ in range(args.epochs * args.iters_per_epoch - 1 if name == 'polynomiallr' else args.epochs):
+        traj.append([g['lr'] for g in opt.param_groups])
+        opt.step()
+        sched.step()
+    np.testing.assert_allclose(traj, _host_ref()['lrer'][name], rtol=1e-12)
 
 
 _BASE_CFG = {'lr': 0.00025, 'momentum': 0.9, 'weight_decay': 0.0005, 'epochs': 20, 'log_freq': 10 ** 6,
@@ -380,94 +333,63 @@ _CASES = [(alg, None) for alg in _VALID] + [
 ]
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference tree only exists in the build container')
+TASK_FUNC_HOOKS = ('sslcct_ad_in_channels', 'sslcct_ad_out_channels', 'sslcct_ad_upsample_scale', 'sslgct_fd_in_channels',
+                   'ssladv_fcd_in_channels', 'ssls4l_rc_in_channels')
+
+
 @pytest.mark.parametrize('alg,override', _CASES)
 def test_algorithm_constructors_validate_arguments_like_the_reference(alg, override, capsys):
     """``log_err`` (banner + exit) for the same unset / invalid SSL arguments as the reference's ``__init__`` checks
     (e.g. ssl_mt.py:76-92, ssl_cutmix.py:79-94), acceptance of the shipped-script values."""
     import importlib
-    import sys
-    if '/root/reference' not in sys.path:
-        sys.path.insert(0, '/root/reference')
     from pixelssl_b200 import runner
     cfg = dict(_BASE_CFG, ssl_algorithm=alg, **_VALID[alg])
     cfg.update(override or {})
-    ref_mod = importlib.import_module('pixelssl.ssl_algorithm.' + alg)
     eng_mod = importlib.import_module('pixelssl_b200.ssl_algorithm.' + alg)
     cls = {'ssl_mt': 'SSLMT', 'ssl_cutmix': 'SSLCUTMIX', 'ssl_adv': 'SSLADV', 'ssl_gct': 'SSLGCT', 'ssl_cct': 'SSLCCT'}[alg]
-
-    def rejected(mod):
-        try:
-            getattr(mod, cls)(runner.build_args(dict(cfg), iters_per_epoch=5))
-            return False
-        except SystemExit:
-            return True
-    saved = torch.Tensor.cuda
-    torch.Tensor.cuda = lambda self, *a, **k: self          # the reference's GCT constructor moves a buffer to the GPU
+    want = [r for a, o, r in _host_ref()['constructor_rejects'] if a == alg and o == override]
+    assert len(want) == 1
     try:
-        want = rejected(ref_mod)
-    finally:
-        torch.Tensor.cuda = saved
-    got = rejected(eng_mod)
+        getattr(eng_mod, cls)(runner.build_args(dict(cfg), iters_per_epoch=5))
+        got = False
+    except SystemExit:
+        got = True
     capsys.readouterr()
-    assert got == want, 'reference rejects: %s, engine rejects: %s' % (want, got)
+    assert got == want[0], 'reference rejects: %s, engine rejects: %s' % (want[0], got)
     if override is None:
         assert not got
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference tree only exists in the build container')
 @pytest.mark.parametrize('arch', ['deeplabv2', 'pspnet'])
 def test_task_func_shape_hooks_match_reference(arch):
     """The scalar TaskFunc hooks the algorithms size their auxiliary networks with (task/sseg/func.py:134-253)."""
-    import importlib
-    import sys
-    for p in ('/root/reference', '/root/reference/task/sseg'):
-        if p not in sys.path:
-            sys.path.insert(0, p)
     from pixelssl_b200 import runner
     from pixelssl_b200.task.sseg import func as eng_func
     args = runner.build_args(dict(_BASE_CFG, ssl_algorithm='ssl_cct', models={'model': arch}, im_size=65, **_VALID['ssl_cct']),
                              iters_per_epoch=5)
-    saved = (torch.Tensor.cuda, torch.nn.Module.cuda)
-    torch.Tensor.cuda = lambda self, *a, **k: self
-    torch.nn.Module.cuda = lambda self, *a, **k: self
-    try:
-        ref = importlib.import_module('func').task_func()(args)
-    finally:
-        torch.Tensor.cuda, torch.nn.Module.cuda = saved
     eng = eng_func.task_func()(args)
-    for hook in ('sslcct_ad_in_channels', 'sslcct_ad_out_channels', 'sslcct_ad_upsample_scale', 'sslgct_fd_in_channels',
-                 'ssladv_fcd_in_channels', 'ssls4l_rc_in_channels'):
-        assert getattr(eng, hook)() == getattr(ref, hook)(), hook
-    assert eng.METRIC_STR == ref.METRIC_STR
+    ref = _host_ref()['task_func'][arch]
+    for hook in TASK_FUNC_HOOKS:
+        assert getattr(eng, hook)() == ref[hook], hook
+    assert eng.METRIC_STR == ref['METRIC_STR']
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference tree only exists in the build container')
 @pytest.mark.parametrize('name', ['sgd', 'adam'])
 def test_optimizer_wrappers_build_the_reference_optimizer(name):
     """optimizer export functions (pixelssl/nn/optimizer.py:57-123): same torch optimizer class and the same
     hyper-parameters in every param group, including the defaults behind the parser's -1 placeholders."""
     import argparse
-    import importlib
-    import sys
-    if '/root/reference' not in sys.path:
-        sys.path.insert(0, '/root/reference')
-    ref = importlib.import_module('pixelssl.nn.optimizer')
+    import json
     from pixelssl_b200.nn import optimizer as eng
-
-    def build(mod):
-        parser = argparse.ArgumentParser()
-        mod.add_parser_arguments(parser)
-        args = parser.parse_args(['--lr', '0.00025'])
-        w = [torch.nn.Parameter(torch.zeros(2)), torch.nn.Parameter(torch.zeros(3))]
-        groups = [{'params': [w[0]], 'lr': args.lr}, {'params': [w[1]], 'lr': 10 * args.lr}]
-        return getattr(mod, name)(args)(groups)
-    a, b = build(ref), build(eng)
-    assert type(a) is type(b)
-    for ga, gb in zip(a.param_groups, b.param_groups):
-        ka = {k: v for k, v in ga.items() if k != 'params'}
-        kb = {k: v for k, v in gb.items() if k != 'params'}
-        assert ka == kb
+    parser = argparse.ArgumentParser()
+    eng.add_parser_arguments(parser)
+    args = parser.parse_args(['--lr', '0.00025'])
+    w = [torch.nn.Parameter(torch.zeros(2)), torch.nn.Parameter(torch.zeros(3))]
+    opt = getattr(eng, name)(args)([{'params': [w[0]], 'lr': args.lr}, {'params': [w[1]], 'lr': 10 * args.lr}])
+    ref = _host_ref()['optimizer'][name]
+    assert type(opt).__module__ + '.' + type(opt).__name__ == ref['class']
+    groups = json.loads(json.dumps([{k: v for k, v in g.items() if k != 'params'} for g in opt.param_groups], default=str))
+    assert groups == ref['groups']
 
 
 def test_pretrained_backbone_url_resolution_and_key_filtered_load(tmp_path, monkeypatch):

@@ -1,6 +1,5 @@
-"""Per-shape device timing of the tcgen05 convolution kernels (forward/dgrad kernel and wgrad kernel) on the
-ResNet-101 @ 513x513, batch 16 shapes that dominate the MT step.  Scratch tool for tuning; knobs are read
-from the environment by the library once per process (PXL_TC_SMEM_KB, PXL_TC_BN_MAX_TF32, ...).
+"""Per-shape device timing of the wgmma convolution kernels (forward/dgrad kernel and wgrad kernel) on the
+ResNet-101 @ 513x513, batch 16 shapes that dominate the MT step.
 
     python tools/bench_conv.py tf32|tf32x3|f16x3|f16 [fwd|wgrad|both]
 
@@ -65,7 +64,7 @@ def main():
     what = sys.argv[2] if len(sys.argv) > 2 else 'both'
     prec = ops.PRECISION[prec_name]
     tot_f = tot_w = 0.0
-    print('precision %s   knobs: %s' % (prec_name, {k: v for k, v in os.environ.items() if k.startswith('PXL_TC') or k.startswith('PXL_WG')}))
+    print('precision %s' % prec_name)
     for name, N, H, W, Cin, Cout, k, dil, mult in SHAPES:
         taps = taps_of(k, dil)
         nt = k * k

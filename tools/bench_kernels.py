@@ -28,7 +28,7 @@ def timeit(fn, iters=20, warmup=5, flush=None):
 
 def main():
     dev = 'cuda'
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)    # 256 MB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)    # 256 MB > 50 MB L2
     out = {}
     for rows in (8, 16):
         n = rows * 21 * 513 * 513
