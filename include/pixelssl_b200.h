@@ -401,6 +401,20 @@ int pxl_aspp_gather(const float* Z, const float* bias, float* out, int N, int H,
 int pxl_aspp_scatter_h16(const float* dy, void* hi, void* lo, float* slot, int target_log2, int N, int H, int W, int C,
                          int ldy, int ldz, const int* taps_dydx_host, int ntaps, void* stream);
 
+/* ---- DeepLabV3+ head concatenations (csrc/lane_concat.cu) ----------------------------------------------------
+ * pxl_lane_concat_nhwc: dst [N,H,W,ld] from nsrc (1..8) NHWC sources in one launch.  geo_host holds 5 ints per source,
+ * {h, w, lds, c, off}: lanes [0, c) of source k (h x w pixels, lane stride lds) fill dst lanes [off, off + c), copied
+ * when h x w == H x W and bilinearly resized (align_corners=True) otherwise, so a 1x1 source is broadcast.  Windows
+ * must not overlap; lanes no window covers are written 0.
+ * pxl_lane_concat_bwd_nhwc: grad = gradient of dst; src_grads_host[k] (NULL = not wanted) receives source k's gradient
+ * [N,h,w,lds], lanes >= c zero.  Every value is gathered in a fixed order (no atomics): bit-identical across runs.
+ * pxl_spatial_mean_nhwc: y [N,C] = mean over the H*W pixels of x [N,H,W,C], fp64 sums in a fixed order. */
+int pxl_lane_concat_nhwc(const float* const* srcs_host, const int* geo_host, int nsrc, float* dst, int N, int H, int W,
+                         int ld, void* stream);
+int pxl_lane_concat_bwd_nhwc(const float* grad, float* const* src_grads_host, const int* geo_host, int nsrc, int N, int H,
+                             int W, int ld, void* stream);
+int pxl_spatial_mean_nhwc(const float* x, float* y, int N, int H, int W, int C, void* stream);
+
 /* ---- S4L (pixelssl/ssl_algorithm/ssl_s4l.py) --------------------------------------------------------------
  * SSLS4L._batch_prehandle (:296-350): out [2*bs,C,H,W] = the batch followed by its rotated copies
  * (_rotate_tensor :352-360, angle in {1,2,3} quarter turns per sample; angles = DEVICE int32 [bs]). */

@@ -33,6 +33,7 @@ def register_into_pixelssl(pixelssl_module=None, task_sseg_modules=None):
         task_model, task_criterion = task_sseg_modules[0], task_sseg_modules[1]
         task_model.deeplabv2 = b200_model.deeplabv2
         task_model.pspnet = b200_model.pspnet
+        task_model.deeplabv3plus = b200_model.deeplabv3plus
         task_criterion.sseg_criterion = b200_criterion.sseg_criterion
         if len(task_sseg_modules) > 2:
             # optional third module = the task's func.py: validation metrics on the GPU (confusion matrix kernel);

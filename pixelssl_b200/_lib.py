@@ -114,6 +114,10 @@ SIGNATURES = {
     'pxl_stem_im2col_h16': (c_int, [P, P, P, c_float, c_int, c_int, c_int, c_int, c_int, P]),
     'pxl_aspp_gather': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int), c_int, P]),
     'pxl_aspp_scatter_h16': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int), c_int, P]),
+    'pxl_lane_concat_nhwc': (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_int), c_int, P, c_int, c_int, c_int, c_int, P]),
+    'pxl_lane_concat_bwd_nhwc': (c_int, [P, ctypes.POINTER(c_void_p), ctypes.POINTER(c_int), c_int, c_int, c_int, c_int, c_int,
+                                         P]),
+    'pxl_spatial_mean_nhwc': (c_int, [P, P, c_int, c_int, c_int, c_int, P]),
     'pxl_s4l_rotate_batch': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, P]),
     'pxl_input_prehandle': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, P, c_int, P, P, c_int, c_int, c_int, c_int,
                                     c_int, c_float, c_float, P, P, P, P, P]),

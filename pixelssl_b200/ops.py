@@ -1990,6 +1990,72 @@ def pyramid_concat(features, branches):
     return _PyramidConcat.apply(as_cl(features), *[as_cl(b) for b in branches])
 
 
+class _SpatialMean(torch.autograd.Function):
+    """nn.AdaptiveAvgPool2d(1) on NHWC with the sums taken in a fixed order (csrc/lane_concat.cu).  The backward is the
+    bin-1 adaptive-pool backward, which gathers as well."""
+
+    @staticmethod
+    def forward(ctx, x):
+        _chk(x, 'x', cl=True)
+        n, c, h, w = x.shape
+        y = torch.empty((n, c, 1, 1), dtype=torch.float32, device=x.device, memory_format=CL)
+        _timed_call('pxl_spatial_mean_nhwc', _p(x), _p(y), n, h, w, c, _stream())
+        ctx.meta = (n, c, h, w)
+        return y
+
+    @staticmethod
+    def backward(ctx, g):
+        n, c, h, w = ctx.meta
+        g = as_cl(g)
+        dx = torch.empty((n, c, h, w), dtype=torch.float32, device=g.device, memory_format=CL)
+        call('pxl_adaptive_avgpool_nhwc', _p(g), _p(dx), n, h, w, c, 1, 1, _stream())
+        return dx
+
+
+def spatial_mean(x):
+    """x.mean((2, 3), keepdim=True) of a channels_last tensor, reproducible bit for bit."""
+    return _SpatialMean.apply(as_cl(x))
+
+
+class _LaneConcat(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, size, ld, chans, *srcs):
+        H, W = size
+        n = srcs[0].shape[0]
+        geo, off = [], 0
+        for s, c in zip(srcs, chans):
+            _chk(s, 'source', cl=True)
+            if s.shape[0] != n:
+                raise ValueError('sources differ in batch size')
+            geo += [s.shape[2], s.shape[3], s.shape[1], c, off]
+            off += c
+        out = torch.empty((n, ld, H, W), dtype=torch.float32, device=srcs[0].device, memory_format=CL)
+        ptrs = (ctypes.c_void_p * len(srcs))(*[s.data_ptr() for s in srcs])
+        _timed_call('pxl_lane_concat_nhwc', ptrs, _ctaps(geo), len(srcs), _p(out), n, H, W, ld, _stream())
+        ctx.meta = (n, H, W, ld, geo, [s.shape for s in srcs])
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        n, H, W, ld, geo, shapes = ctx.meta
+        g = as_cl(g)
+        grads = [torch.empty(shp, dtype=torch.float32, device=g.device, memory_format=CL) if ctx.needs_input_grad[3 + i]
+                 else None for i, shp in enumerate(shapes)]
+        ptrs = (ctypes.c_void_p * len(grads))(*[_p(t) for t in grads])
+        _timed_call('pxl_lane_concat_bwd_nhwc', _p(g), ptrs, _ctaps(geo), len(grads), n, H, W, ld, _stream())
+        return (None, None, None) + tuple(grads)
+
+
+def lane_concat(sources, size, ld=None):
+    """torch.cat([F.interpolate(s[:, :c], size, mode='bilinear', align_corners=True) for s, c in sources], 1),
+    zero-padded to ``ld`` channels, as one channels_last tensor.  Each source is a channels_last tensor of which the
+    first ``c`` channels are used; a source of the output size is copied and a 1x1 source is broadcast.  The backward
+    gathers every gradient in a fixed order (no atomics), so it is reproducible bit for bit."""
+    chans = tuple(int(c) for _, c in sources)
+    ld = sum(chans) if ld is None else int(ld)
+    return _LaneConcat.apply((int(size[0]), int(size[1])), ld, chans, *[as_cl(s) for s, _ in sources])
+
+
 def confusion_matrix_(cmat, pred, gt, num_classes=None):
     """cmat[gt*C + argmax(pred,1)] += 1 over pixels with 0 <= gt < C, accumulated in place into the int64
     device tensor ``cmat`` [C,C] (task/sseg/func.py:36-48: np.argmax + np.bincount)."""

@@ -27,6 +27,7 @@ from ..nn import func
 from ..nn.arena import EngineParallel
 from ..nn.modules import Conv2d, PixelShuffle, upsample
 from . import ssl_base
+from ..task.sseg import func as sseg_func
 
 
 def add_parser_arguments(parser):
@@ -268,7 +269,7 @@ class SSLCCT(ssl_base._SSLBase):
         self.criterions = {'criterion': self.criterion, 'cons_criterion': ops.softmax_mse}
         self.main_model = model_funcs[0](args=a)
         arch = (a.models or {'model': 'deeplabv2'})['model']
-        ad_in = {'pspnet': 512, 'deeplabv2': 2048}[arch]              # task/sseg/func.py:222-253
+        ad_in = sseg_func.CCT_AD_IN_CHANNELS[arch]                    # task/sseg/func.py:222-253
         up, nc = 8, a.num_classes
         decoders = [VATDecoder(up, ad_in, nc, xi=a.vat_dec_xi, eps=a.vat_dec_eps) for _ in range(a.vat_dec_num)]
         decoders += [DropOutDecoder(up, ad_in, nc, drop_rate=a.drop_dec_rate, spatial_dropout=a.drop_dec_spatial)

@@ -7,6 +7,10 @@ import torch
 from ... import ops
 
 
+# channels of each task model's ``resulter['sslcct_ad_inp']``
+CCT_AD_IN_CHANNELS = {'pspnet': 512, 'deeplabv2': 2048, 'deeplabv3plus': 2048}
+
+
 def task_func():
     return SemanticSegmentationFunc
 
@@ -39,7 +43,7 @@ class SemanticSegmentationFunc:
 
     def _arch(self, hook):
         arch = (self.args.models or {'model': 'deeplabv2'})['model']
-        if arch not in ('pspnet', 'deeplabv2'):
+        if arch not in CCT_AD_IN_CHANNELS:
             from ...utils import logger
             logger.log_err('In the SSL_CCT algorithm, the task model \'{0}\' is not supported by the hook \'{1}\'\n'
                            .format(arch, hook))
@@ -47,8 +51,8 @@ class SemanticSegmentationFunc:
 
     def sslcct_ad_in_channels(self):
         """Channels of ``resulter['sslcct_ad_inp']`` (task/sseg/func.py:222-236): the PSP feature for pspnet, the
-        backbone latent for deeplabv2."""
-        return {'pspnet': 512, 'deeplabv2': 2048}[self._arch('sslcct_ad_in_channels')]
+        backbone latent for deeplabv2 and deeplabv3plus."""
+        return CCT_AD_IN_CHANNELS[self._arch('sslcct_ad_in_channels')]
 
     def sslcct_ad_out_channels(self):
         return self.args.num_classes

@@ -1,12 +1,12 @@
 """Task-model plugin for semantic segmentation: the contract of task/sseg/model.py:11-125
-(export fns ``deeplabv2()`` / ``pspnet()``, ``cls(args)``, ``.param_groups``,
+(export fns ``deeplabv2()`` / ``pspnet()``, plus ``deeplabv3plus()``, ``cls(args)``, ``.param_groups``,
 ``forward(inp: tuple) -> (resulter, debugger)`` with 'pred', 'activated_pred', 'ssls4l_rc_inp',
 'sslcct_ad_inp')."""
 import torch.nn as nn
 
 from ... import ops
 from ...utils import logger, cmd
-from .module import deeplab_v2, pspnet as pspnet_module
+from .module import deeplab_v2, deeplab_v3plus, pspnet as pspnet_module
 
 
 def add_parser_arguments(parser):
@@ -25,6 +25,10 @@ def deeplabv2():
 
 def pspnet():
     return PSPNet
+
+
+def deeplabv3plus():
+    return DeepLabV3Plus
 
 
 class LazyActivation:
@@ -79,14 +83,15 @@ def pretrained_backbone_url(args):
 
 
 class DeepLabV2(TaskModel):
+    MODULE = deeplab_v2.DeepLabV2
+
     def __init__(self, args):
         super().__init__(args)
         if args.backbone not in ('resnet50', 'resnet101', 'resnet101-coco'):
-            logger.log_err('DeepLabV2 does not support the backbone: {0}\n'.format(args.backbone))
-        self.model = deeplab_v2.DeepLabV2(backbone=args.backbone, output_stride=args.output_stride,
-                                          num_classes=args.num_classes, sync_bn=True,
-                                          freeze_bn=args.freeze_bn,
-                                          pretrained_backbone_url=pretrained_backbone_url(args))
+            logger.log_err('{0} does not support the backbone: {1}\n'.format(type(self).__name__, args.backbone))
+        self.model = self.MODULE(backbone=args.backbone, output_stride=args.output_stride, num_classes=args.num_classes,
+                                 sync_bn=True, freeze_bn=args.freeze_bn,
+                                 pretrained_backbone_url=pretrained_backbone_url(args))
         self.param_groups = [
             {'params': list(self.model.get_1x_lr_params()), 'lr': args.lr},
             {'params': list(self.model.get_10x_lr_params()), 'lr': args.lr * 10},
@@ -103,6 +108,12 @@ class DeepLabV2(TaskModel):
         resulter['ssls4l_rc_inp'] = pred
         resulter['sslcct_ad_inp'] = latent
         return resulter, debugger
+
+
+class DeepLabV3Plus(DeepLabV2):
+    """DeepLabV3+ with the DeepLabV2 plugin surface: same backbones, resulter keys and latent (the layer4 output);
+    backbone at 1x lr, ASPP, decoder and classifier at 10x."""
+    MODULE = deeplab_v3plus.DeepLabV3Plus
 
 
 class PSPNet(TaskModel):

@@ -94,6 +94,13 @@ class ResNet(nn.Module):
         x = self.layer3(x)
         return self.layer4(x)
 
+    def forward_low_level(self, img):
+        """-> (layer1 output [N,256,H/4,W/4], layer4 output): the low-level features a DeepLabV3+ decoder reads."""
+        x = ops.stem_conv(img, self.conv1.weight, want_bn_stats=self.training)
+        x = self.bn1(x, relu=True)
+        low = self.layer1(ops.maxpool3x3s2(x))
+        return low, self.layer4(self.layer3(self.layer2(low)))
+
     def _init_weight(self):
         for m in self.modules():
             if isinstance(m, Conv2d):
