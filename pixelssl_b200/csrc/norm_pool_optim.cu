@@ -244,7 +244,8 @@ extern "C" int pxl_bn_apply_h16(const float* x, const float* scale, const float*
 // from the fp64 sums) + apply.  The CTAs of row block 0 also store mean / inv_std / scale / shift for the backward
 // and update the running statistics.  Same 2-D decomposition as bn_bwd_dx_kernel.
 // ------------------------------------------------------------------------------------------
-// BN_PRE: rows whose loads are issued before the per-channel prologue (0 or 2; registers: 4 CTAs of 256 threads per SM)
+// BN_PRE: rows whose loads are issued before the per-channel prologue (launched with 2; registers: 4 CTAs of 256 threads
+// per SM)
 template <bool RES, bool RELU, int BN_PRE>
 __global__ void __launch_bounds__(256, 4)
 bn_finalize_apply_kernel(const float4* __restrict__ x, const double* __restrict__ sums, double count, double inv_count,
@@ -324,13 +325,6 @@ bn_finalize_apply_kernel(const float4* __restrict__ x, const double* __restrict_
     if (clipped && sat) atomicAdd(sat, 1);
 }
 
-// PXL_BN_PREFETCH (default 2; 0 = loads after the prologue): A/B switch of the first-trip prefetch
-static int bn_prefetch_rows() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("PXL_BN_PREFETCH"); v = e ? atoi(e) : 2; }
-    return v;
-}
-
 static RedLayout stream_layout(int64_t rows, int C) {
     RedLayout L;
     const int c4 = C / 4;
@@ -380,10 +374,10 @@ extern "C" int pxl_bn_finalize_apply_h16(const float* x, const double* sums, dou
 #define PXL_FA_ARGS (const float4*)x, sums, count, 1.0 / count, gamma, beta, running_mean, running_var, momentum, eps, clamp_mode, mean, invstd, \
                     scale, shift, (const float4*)residual, (float4*)y, rows, C, L.TX, L.TY, L.rowsPerBlock, \
                     (uint2*)hi, (uint2*)lo, hscale, sat, (uint8_t*)relu_mask
-    if (residual && relu) { if (bn_prefetch_rows()) pxl_launch_pdl(bn_finalize_apply_kernel<true, true, 2>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS); else pxl_launch_pdl(bn_finalize_apply_kernel<true, true, 0>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS); }
-    else if (residual) { if (bn_prefetch_rows()) pxl_launch_pdl(bn_finalize_apply_kernel<true, false, 2>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS); else pxl_launch_pdl(bn_finalize_apply_kernel<true, false, 0>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS); }
-    else if (relu) { if (bn_prefetch_rows()) pxl_launch_pdl(bn_finalize_apply_kernel<false, true, 2>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS); else pxl_launch_pdl(bn_finalize_apply_kernel<false, true, 0>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS); }
-    else { if (bn_prefetch_rows()) pxl_launch_pdl(bn_finalize_apply_kernel<false, false, 2>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS); else pxl_launch_pdl(bn_finalize_apply_kernel<false, false, 0>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS); }
+    if (residual && relu) pxl_launch_pdl(bn_finalize_apply_kernel<true, true, 2>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS);
+    else if (residual) pxl_launch_pdl(bn_finalize_apply_kernel<true, false, 2>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS);
+    else if (relu) pxl_launch_pdl(bn_finalize_apply_kernel<false, true, 2>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS);
+    else pxl_launch_pdl(bn_finalize_apply_kernel<false, false, 2>, dim3(grid), dim3(256), 0, st, PXL_FA_ARGS);
 #undef PXL_FA_ARGS
     PXL_CHECK_LAUNCH();
     return 0;
@@ -627,14 +621,14 @@ extern "C" int pxl_bn_bwd_dx_h16(const float* x, const float* y, const float* dy
 #define PXL_DX_ARGS x4, y4, d4, mean, invstd, gamma, dsums, ic, o4, r4, rows, C, L.TX, L.TY, L.rowsPerBlock, scale, shift, \
                     (dgamma_acc && dbeta_acc) ? dgamma_acc : nullptr, dbeta_acc, (uint2*)dhi, (uint2*)dlo, slot, target_log2, sat, (const uint8_t*)relu_mask
     const int mode = relu ? (relu_mask ? 3 : (y ? 1 : 2)) : 0;
-    if (mode == 3 && dres) { if (bn_prefetch_rows()) pxl_launch_pdl(bn_bwd_dx_kernel<3, true, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); else pxl_launch_pdl(bn_bwd_dx_kernel<3, true, 0>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); }
-    else if (mode == 3) { if (bn_prefetch_rows()) pxl_launch_pdl(bn_bwd_dx_kernel<3, false, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); else pxl_launch_pdl(bn_bwd_dx_kernel<3, false, 0>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); }
-    else if (mode == 1 && dres) { if (bn_prefetch_rows()) pxl_launch_pdl(bn_bwd_dx_kernel<1, true, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); else pxl_launch_pdl(bn_bwd_dx_kernel<1, true, 0>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); }
-    else if (mode == 1) { if (bn_prefetch_rows()) pxl_launch_pdl(bn_bwd_dx_kernel<1, false, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); else pxl_launch_pdl(bn_bwd_dx_kernel<1, false, 0>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); }
-    else if (mode == 2 && dres) { if (bn_prefetch_rows()) pxl_launch_pdl(bn_bwd_dx_kernel<2, true, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); else pxl_launch_pdl(bn_bwd_dx_kernel<2, true, 0>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); }
-    else if (mode == 2) { if (bn_prefetch_rows()) pxl_launch_pdl(bn_bwd_dx_kernel<2, false, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); else pxl_launch_pdl(bn_bwd_dx_kernel<2, false, 0>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); }
-    else if (dres) { if (bn_prefetch_rows()) pxl_launch_pdl(bn_bwd_dx_kernel<0, true, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); else pxl_launch_pdl(bn_bwd_dx_kernel<0, true, 0>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); }
-    else { if (bn_prefetch_rows()) pxl_launch_pdl(bn_bwd_dx_kernel<0, false, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); else pxl_launch_pdl(bn_bwd_dx_kernel<0, false, 0>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS); }
+    if (mode == 3 && dres) pxl_launch_pdl(bn_bwd_dx_kernel<3, true, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS);
+    else if (mode == 3) pxl_launch_pdl(bn_bwd_dx_kernel<3, false, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS);
+    else if (mode == 1 && dres) pxl_launch_pdl(bn_bwd_dx_kernel<1, true, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS);
+    else if (mode == 1) pxl_launch_pdl(bn_bwd_dx_kernel<1, false, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS);
+    else if (mode == 2 && dres) pxl_launch_pdl(bn_bwd_dx_kernel<2, true, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS);
+    else if (mode == 2) pxl_launch_pdl(bn_bwd_dx_kernel<2, false, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS);
+    else if (dres) pxl_launch_pdl(bn_bwd_dx_kernel<0, true, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS);
+    else pxl_launch_pdl(bn_bwd_dx_kernel<0, false, 2>, dim3(grid), dim3(256), 0, st, PXL_DX_ARGS);
 #undef PXL_DX_ARGS
     PXL_CHECK_LAUNCH();
     return 0;

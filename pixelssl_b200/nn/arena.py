@@ -117,7 +117,6 @@ class ParamArena:
         return seg.view(p.shape)
 
     def zero_grad(self):
-        ops.join_side_streams()
         ops.new_step()
         self.grad.zero_()
         for p, o in zip(self.params, self.offsets):
@@ -138,7 +137,6 @@ class ParamArena:
 
     def all_reduce_grads(self, group=None):
         import torch.distributed as dist
-        ops.join_side_streams()           # weight gradients launched on the side stream are complete from here on
         if self.distributed and dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
             if dist.get_backend(group) == 'nccl':
                 dist.all_reduce(self.grad, op=dist.ReduceOp.AVG, group=group)     # the 1/world scaling rides in the reduction
@@ -150,7 +148,6 @@ class ParamArena:
         """torch.optim.SGD.step() semantics (momentum, weight decay, dampening 0, no nesterov) read
         from ``optimizer.param_groups`` (so LR schedulers keep working), fused with the teacher
         EMA (ssl_mt.py:359-363) when ``teacher`` (a ParamArena with identical layout) is given."""
-        ops.join_side_streams()
         if self.mom is None:
             self.mom = torch.zeros_like(self.data)
         first = self.steps == 0
@@ -174,7 +171,6 @@ class ParamArena:
     def adam_step(self, optimizer):
         """torch.optim.Adam.step() semantics (no amsgrad) on the flat arena: the FC discriminator /
         flaw detector optimiser (ssl_adv.py:101-102, ssl_gct.py:153-154)."""
-        ops.join_side_streams()
         if getattr(self, 'exp_avg', None) is None:
             self.exp_avg = torch.zeros_like(self.data)
             self.exp_avg_sq = torch.zeros_like(self.data)

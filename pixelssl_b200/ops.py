@@ -8,12 +8,13 @@ Conventions
     reference; labels: float [n,1,H,W] holding integers (task/sseg/data.py:179-182).
 All tensors must be fp32 CUDA tensors; anything else raises (no silent fallback)."""
 import ctypes
-import os as _os
+import functools
 
 import torch
 
 from . import _lib
 from ._lib import ConvGeom, ConvTcExt, call
+from .nn.peer import MAX_VALUES as _PEER_MAX_VALUES
 
 CL = torch.channels_last
 # conv precision policy (pxl_conv_geom.precision): 0 fp32 FFMA, 1 TF32 wgmma, 2 3xTF32 wgmma,
@@ -24,7 +25,6 @@ H16_ACT_SCALE = 16.0            # fixed power-of-two scales of fp16 pairs (csrc/
 H16_W_SCALE = 256.0             # beyond +-4094, weights beyond +-255 (counted: h16_status())
 H16_GRAD_TARGET_LOG2 = 14       # gradients: per-tensor scale putting the absmax in (2^13, 2^14]
 _conv_precision = 0
-_WGRAD_TC_STRIDES = (1, 2)      # convolution strides the wgmma wgrad kernel handles
 
 
 def set_conv_precision(name):
@@ -341,10 +341,14 @@ def _ctaps(t):
     return (ctypes.c_int * len(t))(*t)
 
 
+def _conv_geometry(H, W, kh, kw, stride, padding, dilation):
+    """-> (OH, OW, taps) of an nn.Conv2d-style convolution."""
+    OH = (H + 2 * padding - dilation * (kh - 1) - 1) // stride + 1
+    OW = (W + 2 * padding - dilation * (kw - 1) - 1) // stride + 1
+    return OH, OW, _taps(kh, kw, dilation, padding)
+
+
 _epoch = 0
-ACCUM_WGRAD_INPLACE = True      # wgrad kernels add straight into weight.grad (the flat gradient arena)
-FUSE_BN_FINALIZE = _os.environ.get('PXL_BN_FUSED_FINALIZE', '1') != '0'     # finalize inside the apply launch
-BATCH_WEIGHT_PREP = _os.environ.get('PXL_BATCH_WEIGHT_PREP', '1') != '0'    # arena-wide weight transposes / tf32 splits
 
 
 def new_step():
@@ -425,22 +429,21 @@ def split_tf32(x):
     return hi, lo
 
 
-def split_cached(x):
-    """split_tf32 memoised on the tensor object (an activation feeding two convolutions, a weight
-    used by several launches of one step).  Invalidated by in-place edits and by new_step()."""
-    arena, off = _arena_of(x) if (x.dim() == 4 and BATCH_WEIGHT_PREP) else (None, None)
-    if arena is not None and off in arena._conv_at:
-        n = x.numel()
-        return arena.derived('hi')[off:off + n], arena.derived('lo')[off:off + n]
-    ent = getattr(x, '_pxl_parts', None)
-    if ent is not None and ent[0] == _epoch and ent[1] == x._version and ent[2] == x.data_ptr():
+def _step_get(t, attr):
+    """What _step_put memoised on tensor ``t`` under ``attr``, or None once it is stale: after new_step() or an
+    in-place edit of t."""
+    ent = getattr(t, attr, None)
+    if ent is not None and ent[0] == _epoch and ent[1] == t._version and ent[2] == t.data_ptr():
         return ent[3]
-    parts = split_tf32(x)
+    return None
+
+
+def _step_put(t, attr, value):
     try:
-        x._pxl_parts = (_epoch, x._version, x.data_ptr(), parts)
+        setattr(t, attr, (_epoch, t._version, t.data_ptr(), value))
     except Exception:
         pass
-    return parts
+    return value
 
 
 class H16:
@@ -501,37 +504,61 @@ def h16_status_sites():
     return tuple(int(v) for v in out)
 
 
-def h16_cached(x, scale, want_lo=True):
-    """h16_split memoised on the tensor object for one step (a weight used by several launches)."""
-    ent = getattr(x, '_pxl_h16', None)
-    if ent is not None and ent[0] == _epoch and ent[1] == x._version and ent[2] == x.data_ptr() and ent[3].has_lo >= want_lo:
-        return ent[3]
-    h = h16_split(x, scale, want_lo)
-    try:
-        x._pxl_h16 = (_epoch, x._version, x.data_ptr(), h)
-    except Exception:
-        pass
-    return h
+def _pair_of(t, want_lo, scale=H16_ACT_SCALE):
+    """The fp16 pair of t: attached by its producer (same step, unmodified), else split now and memoised on t for the
+    step (an activation feeding several convolutions, a weight used by several launches)."""
+    h = _step_get(t, '_pxl_h16')
+    if h is not None and h.has_lo >= want_lo:
+        return h
+    if getattr(t, '_pxl_carrier', False):
+        raise RuntimeError('fp16-pair carrier tensor without a valid pair (stale step?)')
+    return _step_put(t, '_pxl_h16', h16_split(t, scale, want_lo))
 
 
-def h16_weight(w, transposed_of=None):
-    """fp16 pair of a packed conv weight; arena weights are served from the arena-wide pair made once per step."""
-    want_lo = _conv_precision == 3
-    arena, off = _arena_of(w) if (w.dim() == 4 and BATCH_WEIGHT_PREP) else (None, None)
-    if arena is not None and off in arena._conv_at:
+def conv_weight(w, form, shape, transposed=False, want_lo=True):
+    """A packed conv weight [Cout][T][Cin] (``shape`` = (Cout, T, Cin)) in the form a launch reads: 'raw', 'split'
+    (tf32 hi, lo) or 'h16' (fp16 pair at H16_W_SCALE); transposed: [Cin][T][Cout], the dgrad operand.  A weight of a
+    registered parameter arena comes from the arena-wide copy (one launch per step for all weights); any other weight
+    is converted here, its plain split and pair cached on the tensor for the step."""
+    arena, off = _arena_of(w)
+    if arena is not None and arena._conv_at.get(off) == shape:
         n = w.numel()
-        return H16(arena.derived('h16')[:, off:off + n], n, H16_W_SCALE, None, True)
-    return h16_cached(w, H16_W_SCALE, want_lo)
+        if form == 'h16':
+            return H16(arena.derived('h16_t' if transposed else 'h16')[:, off:off + n], n, H16_W_SCALE, None, True)
+        if form == 'split':
+            hi, lo = ('t_hi', 't_lo') if transposed else ('hi', 'lo')
+            return arena.derived(hi)[off:off + n], arena.derived(lo)[off:off + n]
+        return arena.derived('t')[off:off + n] if transposed else w
+    if form == 'h16':
+        if transposed:
+            return h16_split(transpose_weights(w, *shape), H16_W_SCALE, want_lo)
+        return _pair_of(w, want_lo, H16_W_SCALE)
+    if form == 'split':
+        hi, lo = _step_get(w, '_pxl_parts') or _step_put(w, '_pxl_parts', split_tf32(w))
+        return (transpose_weights(hi, *shape), transpose_weights(lo, *shape)) if transposed else (hi, lo)
+    return transpose_weights(w, *shape) if transposed else w
 
 
-def h16_supported(Cin, mul, div):
-    return Cin % 64 == 0 and ((div == 1 and mul in (1, 2)) or (div == 2 and mul == 1))
-
-
-def tc_supported(Cin, mul, div):
-    """Shapes covered by the wgmma forward/dgrad kernel (csrc/conv_tc.cu): stride 1 and 2 forward
-    (mul), and the dgrad of a stride-2 convolution (div == 2, decomposed by output parity)."""
-    return Cin % 32 == 0 and ((div == 1 and mul in (1, 2)) or (div == 2 and mul == 1))
+@functools.lru_cache(maxsize=None)
+def conv_route(direction, Cin, Cout, mul, div, precision):
+    """Kernel family serving a convolution launch -> (family, precision it runs at).  direction: 'fwd' or 'dgrad' (one
+    kernel: a dgrad is a forward launch over dY, that of a stride-2 convolution with div == 2) or 'wgrad'; Cin, Cout:
+    the launch's channel counts (Cout: ldo for a wgrad); mul, div: the launch's stride / dgrad stride.
+    'h16': the fp16-pair wgmma kernels (precision 3, 4) cover channel counts that are multiples of 64, 'tc': the
+    tf32 wgmma kernels (1, 2) multiples of 32; both stride 1 and 2 forward and the dgrad of a stride-2 convolution
+    (decomposed by output parity), and for a wgrad only stride 1 and 2.  Shapes the fp16 kernels do not cover run on
+    the tf32 kernels of the same grade (H16_FALLBACK); everything else on the FFMA kernels ('ffma', 0)."""
+    if direction == 'wgrad':
+        strides_ok, chans = div == 1 and mul in (1, 2), (Cin, Cout)
+    else:
+        strides_ok, chans = (div == 1 and mul in (1, 2)) or (div == 2 and mul == 1), (Cin,)
+    if precision >= 3:
+        if strides_ok and all(c % 64 == 0 for c in chans):
+            return 'h16', precision
+        precision = H16_FALLBACK[precision]
+    if precision != 0 and strides_ok and all(c % 32 == 0 for c in chans):
+        return 'tc', precision
+    return 'ffma', 0
 
 
 def _stride2_dgrad_classes(taps, ntaps):
@@ -550,100 +577,73 @@ def _stride2_dgrad_classes(taps, ntaps):
     return classes
 
 
-def _tc_launch(geom, taps, ext, x_parts, w_parts, bias, out):
-    _timed_call('pxl_conv_tc_launch_ex', ctypes.byref(geom), _ctaps(taps), ctypes.byref(ext) if ext is not None else None,
-                _p(x_parts[0]), _p(x_parts[1]), _p(w_parts[0]), _p(w_parts[1]), _p(bias), _p(out), _stream(),
-                meta=(2.0 * geom.N * geom.OH * geom.OW * geom.Cin * geom.Cout * geom.ntaps,
-                      'fwd/dgrad(tf32) N%d %dx%d Cin%d Cout%d taps%d' % (geom.N, geom.OH, geom.OW, geom.Cin, geom.Cout, geom.ntaps)))
-
-
 def conv_raw(x, w_packed, bias, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div, out=None, precision=None, bn_stats=None,
              accumulate=False):
-    """Launch the NHWC tap-table convolution on raw buffers.  w_packed: [Cout][ntaps][Cin] contiguous.
-    precision 0: FFMA kernel; 1: wgmma single-pass TF32; 2: wgmma 3xTF32 (operands split on the
-    fly).  Shapes the tensor-core kernel does not cover (Cin % 32 != 0, other strides) use the FFMA kernel."""
+    """Launch the NHWC tap-table convolution on raw buffers.  w_packed: [Cout][ntaps][Cin] contiguous, or the form the
+    kernel reads (tf32 split tuple, H16).  The kernel family is conv_route's choice for the shape and precision:
+    precision 0 FFMA; 1 wgmma single-pass TF32; 2 wgmma 3xTF32 (activations split in shared memory, weights here);
+    3 / 4 fp16-pair / single-fp16 wgmma.  bn_stats: the tensor-core epilogue also accumulates sum(y), sum(y^2) per
+    channel into it.  accumulate (fp16 kernels): out += the result."""
     ntaps = len(taps) // 2
-    prec = _conv_precision if precision is None else precision
-    if out is None and not isinstance(x, H16):
-        dev = x[0].device if isinstance(x, tuple) else x.device
-        out = torch.empty((N, ldo, OH, OW), dtype=torch.float32, device=dev, memory_format=CL)
+    family, prec = conv_route('fwd', Cin, Cout, mul, div, _conv_precision if precision is None else precision)
+    if family != 'h16' and (isinstance(x, H16) or isinstance(w_packed, H16)):
+        raise ValueError('fp16-pair operands given for a shape the f16 wgmma kernel does not cover')
+    if out is None:
+        out = torch.empty((N, ldo, OH, OW), dtype=torch.float32, device=(x[0] if isinstance(x, tuple) else x).device,
+                          memory_format=CL)
         if ldo != Cout:
             out.zero_()
-    if prec >= 3 and not h16_supported(Cin, mul, div):
-        if isinstance(x, H16) or isinstance(w_packed, H16):
-            raise ValueError('fp16-pair operands given for a shape the f16 wgmma kernel does not cover')
-        prec = H16_FALLBACK[prec]
-    if prec >= 3:
-        want_lo = prec == 3
-        xh = x if isinstance(x, H16) else h16_cached(x, H16_ACT_SCALE, want_lo)
-        wh = w_packed if isinstance(w_packed, H16) else h16_weight(w_packed)
-        fx, px = xh.inv_scale()
-        fw, pw = wh.inv_scale()
-        if px is not None and pw is not None:
-            raise ValueError('at most one operand may carry a device-side scale')
-        oscale, odev = fx * fw, (px if px is not None else pw)
-        if out is None:
-            out = torch.empty((N, ldo, OH, OW), dtype=torch.float32, device=xh.device, memory_format=CL)
-            if ldo != Cout:
-                out.zero_()
-
-        def launch(geom, tp, ext):
-            ext.out_scale, ext.out_scale_dev = oscale, (odev.data_ptr() if odev is not None else None)
-            ext.out_accumulate = 1 if accumulate else 0
-            _timed_call('pxl_conv_h16_launch', ctypes.byref(geom), _ctaps(tp), ctypes.byref(ext), _p(xh.hi), _p(xh.lo),
-                        _p(wh.hi), _p(wh.lo if want_lo else None), _p(bias), _p(out), _stream(),
-                        meta=(2.0 * geom.N * geom.OH * geom.OW * geom.Cin * min(geom.Cout, Cout) * geom.ntaps,
-                              'fwd/dgrad N%d %dx%d Cin%d Cout%d taps%d mul%d' % (geom.N, geom.OH, geom.OW, geom.Cin, geom.Cout, geom.ntaps, geom.mul)))
-        if div == 1:
-            ext = ConvTcExt(0, None, 0, 0, 0, 0, 0, None)
-            if bn_stats is not None:
-                ext.bn_stats = bn_stats.data_ptr()
-                bn_stats._pxl_filled = True
-            launch(ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, 1, ntaps, prec), taps, ext)
-            return out
-        classes = _stride2_dgrad_classes(taps, ntaps)
-        if any(len(c[3]) == 0 for c in classes):
-            out.zero_()
-        for py, px_, sub, widx in classes:
-            ohs, ows = (OH - py + 1) // 2, (OW - px_ + 1) // 2
-            if not widx or ohs <= 0 or ows <= 0:
-                continue
-            ext = ConvTcExt(ntaps, (ctypes.c_int * len(widx))(*widx), 2, py, px_, OH, OW, None)
-            launch(ConvGeom(N, H, W, Cin, ohs, ows, Cout, ldo, 1, 1, len(widx), prec), sub, ext)
+    if family == 'ffma':
+        if isinstance(x, tuple):
+            x = x[0] + x[1]
+        if isinstance(w_packed, tuple):
+            w_packed = w_packed[0] + w_packed[1]
+        geom = ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, div, ntaps, 0)
+        call('pxl_conv_nhwc', ctypes.byref(geom), _ctaps(taps), _p(x), _p(w_packed), _p(bias), _p(out), _stream())
         return out
-    if prec != 0 and tc_supported(Cin, mul, div):
-        if prec == 2:
-            # activations go in raw: the kernel splits them hi/lo in shared memory; the (small, per-step
-            # cached) weights are split here
-            x_parts = x if isinstance(x, tuple) else (x, None)
-            w_parts = w_packed if isinstance(w_packed, tuple) else split_cached(w_packed)
-        else:
-            x_parts, w_parts = (x, None), (w_packed, None)
-        if div == 1:
-            geom = ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, 1, ntaps, prec)
-            ext = None
-            if bn_stats is not None:      # the epilogue also accumulates sum(y), sum(y^2) per channel
-                ext = ConvTcExt(0, None, 0, 0, 0, 0, 0, ctypes.c_void_p(bn_stats.data_ptr()))
-                bn_stats._pxl_filled = True
-            _tc_launch(geom, taps, ext, x_parts, w_parts, bias, out)
-            return out
+    if div == 1:
+        ext = None
+        if bn_stats is not None or family == 'h16':
+            ext = ConvTcExt(0, None, 0, 0, 0, 0, 0, _p(bn_stats))
+        if bn_stats is not None:
+            bn_stats._pxl_filled = True
+        launches = [(ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, 1, ntaps, prec), taps, ext)]
+    else:
+        launches = []
         classes = _stride2_dgrad_classes(taps, ntaps)
         if any(len(c[3]) == 0 for c in classes):
             out.zero_()
         for py, px, sub, widx in classes:
             ohs, ows = (OH - py + 1) // 2, (OW - px + 1) // 2
-            if not widx or ohs <= 0 or ows <= 0:
-                continue
-            geom = ConvGeom(N, H, W, Cin, ohs, ows, Cout, ldo, 1, 1, len(widx), prec)
-            ext = ConvTcExt(ntaps, (ctypes.c_int * len(widx))(*widx), 2, py, px, OH, OW, None)
-            _tc_launch(geom, sub, ext, x_parts, w_parts, bias, out)
+            if widx and ohs > 0 and ows > 0:
+                launches.append((ConvGeom(N, H, W, Cin, ohs, ows, Cout, ldo, 1, 1, len(widx), prec), sub,
+                                 ConvTcExt(ntaps, (ctypes.c_int * len(widx))(*widx), 2, py, px, OH, OW, None)))
+    if family == 'h16':
+        want_lo = prec == 3
+        xh = x if isinstance(x, H16) else _pair_of(x, want_lo)
+        wh = w_packed if isinstance(w_packed, H16) else conv_weight(w_packed, 'h16', (Cout, ntaps, Cin), want_lo=want_lo)
+        fx, px = xh.inv_scale()
+        fw, pw = wh.inv_scale()
+        if px is not None and pw is not None:
+            raise ValueError('at most one operand may carry a device-side scale')
+        oscale, odev = fx * fw, _p(px if px is not None else pw)
+        for geom, tp, ext in launches:
+            ext.out_scale, ext.out_scale_dev, ext.out_accumulate = oscale, odev, 1 if accumulate else 0
+            _timed_call('pxl_conv_h16_launch', ctypes.byref(geom), _ctaps(tp), ctypes.byref(ext), _p(xh.hi), _p(xh.lo),
+                        _p(wh.hi), _p(wh.lo if want_lo else None), _p(bias), _p(out), _stream(),
+                        meta=(2.0 * geom.N * geom.OH * geom.OW * geom.Cin * geom.Cout * geom.ntaps,
+                              'fwd/dgrad N%d %dx%d Cin%d Cout%d taps%d mul%d' % (geom.N, geom.OH, geom.OW, geom.Cin, geom.Cout, geom.ntaps, geom.mul)))
         return out
-    if isinstance(x, tuple):
-        x = x[0] + x[1]
-    if isinstance(w_packed, tuple):
-        w_packed = w_packed[0] + w_packed[1]
-    geom = ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, div, ntaps, 0)
-    call('pxl_conv_nhwc', ctypes.byref(geom), _ctaps(taps), _p(x), _p(w_packed), _p(bias), _p(out), _stream())
+    x_parts = x if isinstance(x, tuple) else (x, None)
+    if prec == 2:
+        w_parts = w_packed if isinstance(w_packed, tuple) else conv_weight(w_packed, 'split', (Cout, ntaps, Cin))
+    else:
+        w_parts = (w_packed, None)
+    for geom, tp, ext in launches:
+        _timed_call('pxl_conv_tc_launch_ex', ctypes.byref(geom), _ctaps(tp), ctypes.byref(ext) if ext is not None else None,
+                    _p(x_parts[0]), _p(x_parts[1]), _p(w_parts[0]), _p(w_parts[1]), _p(bias), _p(out), _stream(),
+                    meta=(2.0 * geom.N * geom.OH * geom.OW * geom.Cin * geom.Cout * geom.ntaps,
+                          'fwd/dgrad(tf32) N%d %dx%d Cin%d Cout%d taps%d' % (geom.N, geom.OH, geom.OW, geom.Cin, geom.Cout, geom.ntaps)))
     return out
 
 
@@ -655,12 +655,11 @@ def conv_tc_status():
 def conv_wgrad_raw(x, dy, dw, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div, precision=None):
     """dw[Cout][ntaps][Cin] += ...  (dw must be initialised by the caller)."""
     ntaps = len(taps) // 2
-    prec = _conv_precision if precision is None else precision
-    if prec >= 3 and not (div == 1 and mul in _WGRAD_TC_STRIDES and Cin % 64 == 0 and ldo % 64 == 0):
-        if isinstance(x, H16) or isinstance(dy, H16):
-            raise ValueError('fp16-pair operands given for a shape the f16 wgmma wgrad kernel does not cover')
-        prec = H16_FALLBACK[prec]
-    if prec >= 3:
+    family, prec = conv_route('wgrad', Cin, ldo, mul, div, _conv_precision if precision is None else precision)
+    if family != 'h16' and (isinstance(x, H16) or isinstance(dy, H16)):
+        raise ValueError('fp16-pair operands given for a shape the f16 wgmma wgrad kernel does not cover')
+    geom = ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, div, ntaps, prec)
+    if family == 'h16':
         want_lo = prec == 3
         xh = x if isinstance(x, H16) else h16_split(x, H16_ACT_SCALE, want_lo)
         dh = dy if isinstance(dy, H16) else h16_split(dy, None, want_lo)
@@ -668,31 +667,23 @@ def conv_wgrad_raw(x, dy, dw, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div, p
         fd, pd = dh.inv_scale()
         if px is not None and pd is not None:
             raise ValueError('at most one operand may carry a device-side scale')
-        geom = ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, div, ntaps, prec)
         _timed_call('pxl_conv_wgrad_h16_launch', ctypes.byref(geom), _ctaps(taps), _p(xh.hi), _p(xh.lo), _p(dh.hi), _p(dh.lo),
                     _p(dw), float(fx * fd), _p(pd if pd is not None else px), _stream(),
                     meta=(2.0 * N * OH * OW * Cin * Cout * ntaps, 'wgrad N%d %dx%d Cin%d Cout%d taps%d mul%d' % (N, OH, OW, Cin, Cout, ntaps, mul)))
-        return dw
-    if prec != 0 and div == 1 and mul in _WGRAD_TC_STRIDES and Cin % 32 == 0 and ldo % 32 == 0:
-        geom = ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, div, ntaps, prec)
-        if prec == 2:
-            if isinstance(x, tuple) != isinstance(dy, tuple):        # mixed: split the raw one too
-                x = x if isinstance(x, tuple) else split_tf32(x)
-                dy = dy if isinstance(dy, tuple) else split_tf32(dy)
-            x_hi, x_lo = x if isinstance(x, tuple) else (x, None)     # raw operands: split inside the kernel
-            d_hi, d_lo = dy if isinstance(dy, tuple) else (dy, None)
-            _timed_call('pxl_conv_wgrad_tc_launch', ctypes.byref(geom), _ctaps(taps), _p(x_hi), _p(x_lo), _p(d_hi), _p(d_lo),
-                        _p(dw), _stream(), meta=(2.0 * N * OH * OW * Cin * Cout * ntaps, 'wgrad(tf32) N%d %dx%d Cin%d Cout%d taps%d' % (N, OH, OW, Cin, Cout, ntaps)))
-        else:
-            _timed_call('pxl_conv_wgrad_tc_launch', ctypes.byref(geom), _ctaps(taps), _p(x), _p(None), _p(dy), _p(None),
-                        _p(dw), _stream(), meta=(2.0 * N * OH * OW * Cin * Cout * ntaps, 'wgrad(tf32) N%d %dx%d Cin%d Cout%d taps%d' % (N, OH, OW, Cin, Cout, ntaps)))
-        return dw
-    if isinstance(x, tuple):
-        x = x[0] + x[1]
-    if isinstance(dy, tuple):
-        dy = dy[0] + dy[1]
-    geom = ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, div, ntaps, 0)     # FFMA split-K kernel
-    call('pxl_conv_wgrad_nhwc', ctypes.byref(geom), _ctaps(taps), _p(x), _p(dy), _p(dw), _stream())
+    elif family == 'tc':
+        if prec == 2 and isinstance(x, tuple) != isinstance(dy, tuple):        # mixed: split the raw one too
+            x = x if isinstance(x, tuple) else split_tf32(x)
+            dy = dy if isinstance(dy, tuple) else split_tf32(dy)
+        x_hi, x_lo = x if isinstance(x, tuple) else (x, None)     # raw operands: 3xTF32 splits them inside the kernel
+        d_hi, d_lo = dy if isinstance(dy, tuple) else (dy, None)
+        _timed_call('pxl_conv_wgrad_tc_launch', ctypes.byref(geom), _ctaps(taps), _p(x_hi), _p(x_lo), _p(d_hi), _p(d_lo),
+                    _p(dw), _stream(), meta=(2.0 * N * OH * OW * Cin * Cout * ntaps, 'wgrad(tf32) N%d %dx%d Cin%d Cout%d taps%d' % (N, OH, OW, Cin, Cout, ntaps)))
+    else:
+        if isinstance(x, tuple):
+            x = x[0] + x[1]
+        if isinstance(dy, tuple):
+            dy = dy[0] + dy[1]
+        call('pxl_conv_wgrad_nhwc', ctypes.byref(geom), _ctaps(taps), _p(x), _p(dy), _p(dw), _stream())     # FFMA split-K
     return dw
 
 
@@ -703,127 +694,69 @@ def transpose_weights(w_packed, Cout, T, Cin):
 
 
 class _Conv2d(torch.autograd.Function):
-    """nn.Conv2d on NHWC (resnet.py:18-25 etc.).  weight logical [Cout,Cin,kh,kw] channels_last."""
+    """nn.Conv2d on NHWC (resnet.py:18-25 etc.).  weight logical [Cout,Cin,kh,kw] channels_last.  out_lanes > Cout: the
+    output has that many channel lanes, the extra ones zero, so that the consumer can be a tensor-core convolution
+    with Cin % 32 == 0 (the 21-channel decoder heads)."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, stride, padding, dilation, out_lanes=0, bn_stats=None):
         _chk(x, 'x', cl=True); _chk(weight, 'weight', cl=True)
         N, Cin, H, W = x.shape
         Cout, Cin2, kh, kw = weight.shape
-        if out_lanes and out_lanes > Cout:
-            return _Conv2d._forward_padded(ctx, x, weight, bias, stride, padding, dilation, out_lanes)
-        ctx.padded = False
         if Cin2 != Cin:
             raise ValueError('channel mismatch')
-        OH = (H + 2 * padding - dilation * (kh - 1) - 1) // stride + 1
-        OW = (W + 2 * padding - dilation * (kw - 1) - 1) // stride + 1
-        taps = _taps(kh, kw, dilation, padding)
-        ctx.split, ctx.h16 = False, None
-        ctx.meta = (taps, N, H, W, Cin, OH, OW, Cout, stride, kh * kw, bias is not None)
-        if _conv_precision >= 3 and h16_supported(Cin, stride, 1):
+        ldo = max(out_lanes, Cout)
+        OH, OW, taps = _conv_geometry(H, W, kh, kw, stride, padding, dilation)
+        ctx.h16 = None
+        ctx.meta = (taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, kh * kw, bias is not None)
+        prec = _conv_precision
+        if ldo == Cout and conv_route('fwd', Cin, Cout, stride, 1, prec)[0] == 'h16':
             # fp16-pair path: the pair of x (4 B/element, like x itself) is what the backward keeps
-            xh = h16_cached(x, H16_ACT_SCALE, _conv_precision == 3)
+            xh = _pair_of(x, prec == 3)
             out = conv_raw(xh, weight, bias, taps, N, H, W, Cin, OH, OW, Cout, Cout, stride, 1, bn_stats=bn_stats)
-            wg_ok = Cin % 64 == 0 and Cout % 64 == 0 and stride in _WGRAD_TC_STRIDES
-            if wg_ok or not ctx.needs_input_grad[1]:
+            if conv_route('wgrad', Cin, Cout, stride, 1, prec)[0] == 'h16' or not ctx.needs_input_grad[1]:
                 ctx.save_for_backward(xh.buf, weight)
                 ctx.h16 = (xh.scale, xh.has_lo)
             else:
                 ctx.save_for_backward(x, weight)
             return out
-        out = conv_raw(x, weight, bias, taps, N, H, W, Cin, OH, OW, Cout, Cout, stride, 1, bn_stats=bn_stats)
+        out = conv_raw(x, weight, bias, taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, 1, bn_stats=bn_stats)
         ctx.save_for_backward(x, weight)
         return out
-
-    @staticmethod
-    def _forward_padded(ctx, x, weight, bias, stride, padding, dilation, ldo):
-        """Output written with ``ldo`` > Cout channel lanes (extra lanes zero) so that the consumer can be
-        a tensor-core convolution with Cin % 32 == 0.  Used by the 21-channel decoder heads."""
-        N, Cin, H, W = x.shape
-        Cout, _, kh, kw = weight.shape
-        OH = (H + 2 * padding - dilation * (kh - 1) - 1) // stride + 1
-        OW = (W + 2 * padding - dilation * (kw - 1) - 1) // stride + 1
-        taps = _taps(kh, kw, dilation, padding)
-        out = conv_raw(x, weight, bias, taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, 1)
-        ctx.save_for_backward(x, weight)
-        ctx.padded, ctx.split = True, False
-        ctx.meta = (taps, N, H, W, Cin, OH, OW, Cout, stride, kh * kw, bias is not None, ldo)
-        return out
-
-    @staticmethod
-    def _backward_padded(ctx, dy):
-        x, weight = ctx.saved_tensors
-        taps, N, H, W, Cin, OH, OW, Cout, stride, T, has_bias, ldo = ctx.meta
-        dy = as_cl(dy)                       # [N, ldo, OH, OW]; lanes >= Cout carry zeros
-        dx = dw = db = None
-        if ctx.needs_input_grad[0]:
-            wp = torch.zeros((ldo, T, Cin), dtype=torch.float32, device=dy.device)
-            wp[:Cout] = weight.permute(0, 2, 3, 1).reshape(Cout, T, Cin)
-            wt = transpose_weights(wp, ldo, T, Cin)
-            dx = conv_raw(dy, wt, None, [-v for v in taps], N, OH, OW, ldo, H, W, Cin, Cin, 1, stride)
-        if ctx.needs_input_grad[1]:
-            dwp = torch.zeros((Cout, T, Cin), dtype=torch.float32, device=dy.device)
-            conv_wgrad_raw(x, dy, dwp, taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, 1)
-            kh = int(round(T ** 0.5))
-            dw = dwp.reshape(Cout, kh, T // kh, Cin).permute(0, 3, 1, 2)
-        if has_bias and ctx.needs_input_grad[2]:
-            db = torch.empty(Cout, dtype=torch.float32, device=dy.device)
-            call('pxl_bias_grad', _p(dy), N * OH * OW, Cout, ldo, _p(db), 0, _stream())
-        return dx, dw, db, None, None, None, None, None
 
     @staticmethod
     def backward(ctx, dy):
-        if ctx.padded:
-            return _Conv2d._backward_padded(ctx, dy)
-        if ctx.split:
-            x_hi, x_lo, weight = ctx.saved_tensors
-            x = (x_hi, x_lo)
-        else:
-            x, weight = ctx.saved_tensors
-        taps, N, H, W, Cin, OH, OW, Cout, stride, T, has_bias = ctx.meta
-        dy = as_cl(dy)
+        x, weight = ctx.saved_tensors
+        taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, T, has_bias = ctx.meta
+        dy = as_cl(dy)                       # [N, ldo, OH, OW]; lanes >= Cout carry zeros
         dx = dw = db = None
-        dyin = dy
         if ctx.h16 is not None:
             x = H16(x, x.shape[1], ctx.h16[0], None, ctx.h16[1])
         prec = _conv_precision
-        if prec >= 3:
-            dgrad_h16 = ctx.needs_input_grad[0] and h16_supported(Cout, 1, stride)
-            wgrad_h16 = ctx.needs_input_grad[1] and isinstance(x, H16)
-            if dgrad_h16 or wgrad_h16:
-                dyin = h16_split(dy, None, prec == 3)        # one pair of dY serves dgrad and wgrad
-        eff = H16_FALLBACK.get(prec, prec)
+        dfamily, dprec = conv_route('dgrad', ldo, Cin, 1, stride, prec)
+        dgrad_h16 = ctx.needs_input_grad[0] and ldo == Cout and dfamily == 'h16'
+        dyin = dy
+        if dgrad_h16 or (ctx.needs_input_grad[1] and isinstance(x, H16)):
+            dyin = h16_split(dy, None, prec == 3)        # one pair of dY serves dgrad and wgrad
         if ctx.needs_input_grad[0]:
-            want_split = eff == 2 and tc_supported(Cout, 1, stride)
-            arena, off = _arena_of(weight) if BATCH_WEIGHT_PREP else (None, None)
-            if isinstance(dyin, H16) and h16_supported(Cout, 1, stride):
-                if arena is not None and arena._conv_at.get(off) == (Cout, T, Cin):
-                    n = weight.numel()
-                    wt = H16(arena.derived('h16_t')[:, off:off + n], n, H16_W_SCALE, None, True)
-                else:
-                    wt = h16_split(transpose_weights(weight, Cout, T, Cin), H16_W_SCALE, prec == 3)
-            elif arena is not None and arena._conv_at.get(off) == (Cout, T, Cin):
-                n = weight.numel()          # arena-wide transposed (and split) copies: one launch per step each
-                if want_split:
-                    wt = (arena.derived('t_hi')[off:off + n], arena.derived('t_lo')[off:off + n])
-                else:
-                    wt = arena.derived('t')[off:off + n]
-            elif want_split:
-                w_hi, w_lo = split_cached(weight)
-                wt = (transpose_weights(w_hi, Cout, T, Cin), transpose_weights(w_lo, Cout, T, Cin))
+            if ldo != Cout:
+                wp = torch.zeros((ldo, T, Cin), dtype=torch.float32, device=dy.device)
+                wp[:Cout] = weight.permute(0, 2, 3, 1).reshape(Cout, T, Cin)
+                wt = transpose_weights(wp, ldo, T, Cin)
             else:
-                wt = transpose_weights(weight, Cout, T, Cin)
-            ntaps = [-v for v in taps]
-            dgrad_in = dyin if (isinstance(dyin, H16) and isinstance(wt, H16)) else dy
-            dx = conv_raw(dgrad_in, wt, None, ntaps, N, OH, OW, Cout, H, W, Cin, Cin, 1, stride)
+                form = 'h16' if dgrad_h16 else 'split' if (dfamily, dprec) == ('tc', 2) else 'raw'
+                wt = conv_weight(weight, form, (Cout, T, Cin), transposed=True, want_lo=prec == 3)
+            dx = conv_raw(dyin if dgrad_h16 else dy, wt, None, [-v for v in taps], N, OH, OW, ldo, H, W, Cin, Cin, 1, stride)
         if ctx.needs_input_grad[1]:
-            inplace = ACCUM_WGRAD_INPLACE and weight.grad is not None and weight.grad.is_contiguous(memory_format=CL)
+            # the wgrad kernels add straight into weight.grad (the flat gradient arena); a zero-padded head's gradient
+            # goes through autograd
+            inplace = ldo == Cout and weight.grad is not None and weight.grad.is_contiguous(memory_format=CL)
             dwbuf = weight.grad if inplace else torch.zeros_like(weight, memory_format=torch.preserve_format)
-            conv_wgrad_raw(x, dyin if isinstance(x, H16) else dy, dwbuf, taps, N, H, W, Cin, OH, OW, Cout, Cout, stride, 1)
+            conv_wgrad_raw(x, dyin if isinstance(x, H16) else dy, dwbuf, taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, 1)
             dw = None if inplace else dwbuf
         if has_bias and ctx.needs_input_grad[2]:
             db = torch.empty(Cout, dtype=torch.float32, device=dy.device)
-            call('pxl_bias_grad', _p(dy), N * OH * OW, Cout, Cout, _p(db), 0, _stream())
+            call('pxl_bias_grad', _p(dy), N * OH * OW, Cout, ldo, _p(db), 0, _stream())
         return dx, dw, db, None, None, None, None, None
 
 
@@ -955,7 +888,7 @@ class _AsppGemm(torch.autograd.Function):
 
 
 def aspp(x, weights, biases, dilations=(6, 12, 18, 24)):
-    if _conv_precision >= 3 and x.shape[1] % 64 == 0:
+    if conv_route('fwd', x.shape[1], weights[0].shape[0], 1, 1, _conv_precision)[0] == 'h16':
         return _AsppGemm.apply(x, tuple(dilations), *(tuple(weights) + tuple(biases)))
     return _Aspp.apply(x, tuple(dilations), *(tuple(weights) + tuple(biases)))
 
@@ -1049,6 +982,65 @@ def register_peer_exchange(group, exchange):
         _peer_exchanges[id(group)] = exchange
 
 
+def _bn_train_forward(x, sums, rows, C, gamma, beta, running_mean, running_var, momentum, eps, clamp_var, group, coeff,
+                      residual, relu, y, h16_out=()):
+    """Train-mode (Sync)BN once its statistics ``sums`` exist: reduce them over ``group``, finalize (running statistics,
+    mean / invstd / scale / shift into ``coeff``) and apply -> the element count the statistics cover.  Local: one
+    finalize + apply launch.  Group: the peer exchange finalizes as it reduces (NCCL: all-reduce, then a finalize
+    launch), then an apply launch.  h16_out: the (hi, lo, scale, mask) arguments of the fp16-pair apply variants."""
+    count, clamp = float(rows), 1 if clamp_var else 0
+    if group is None:
+        call('pxl_bn_finalize_apply_h16' if h16_out else 'pxl_bn_finalize_apply', _p(x), _p(sums), count, _p(gamma),
+             _p(beta), _p(running_mean), _p(running_var), float(momentum), float(eps), clamp, _p(coeff[0]), _p(coeff[1]),
+             _p(coeff[2]), _p(coeff[3]), _p(residual), int(relu), _p(y), rows, C, *h16_out, _stream())
+        return count
+    import torch.distributed as dist
+    count *= dist.get_world_size(group)
+    clamp = 1     # batchnorm.py:125: the multi-replica path clamps var instead of adding eps
+    px = _peer_exchanges.get(id(group))
+    if px is not None and 2 * C <= _PEER_MAX_VALUES:
+        # NVLink peer-memory exchange fused with the finalize (csrc/peer_exchange.cu)
+        px.allreduce_bn(sums, (count, C, gamma, beta, running_mean, running_var, momentum, eps, clamp,
+                               coeff[0], coeff[1], coeff[2], coeff[3]))
+    else:
+        dist.all_reduce(sums, group=group)
+        call('pxl_bn_finalize', _p(sums), count, C, _p(gamma), _p(beta), _p(running_mean), _p(running_var),
+             float(momentum), float(eps), clamp, _p(coeff[0]), _p(coeff[1]), _p(coeff[2]), _p(coeff[3]), _stream())
+    call('pxl_bn_apply_h16' if h16_out else 'pxl_bn_apply', _p(x), _p(coeff[2]), _p(coeff[3]), _p(residual), int(relu),
+         _p(y), rows, C, *h16_out, _stream())
+    return count
+
+
+def _bn_backward_sums(dsums, C, gamma, beta, group):
+    """Train-mode (Sync)BN backward after its reduce launch.  d(gamma), d(beta) come from the LOCAL sums (data
+    parallelism averages them with the other gradients).  When the gradient arena is in place they are accumulated by a
+    launch that runs anyway: the dx launch (single GPU) or the peer exchange (before it exchanges the sums); otherwise a
+    params launch writes them into tensors returned to autograd.  Then ``dsums`` is all-reduced over ``group``.
+    -> (dgamma, dbeta, gamma_acc, beta_acc): the tensors for autograd (None when accumulated in place) and the
+    accumulators the dx launch adds into (None unless it does)."""
+    grads_in_arena = (gamma.grad is not None and beta.grad is not None
+                      and gamma.grad.is_contiguous() and beta.grad.is_contiguous())
+    px = _peer_exchanges.get(id(group)) if group is not None else None
+    if px is not None and 2 * C > _PEER_MAX_VALUES:
+        px = None
+    acc_inplace = grads_in_arena and group is None
+    acc_in_exchange = grads_in_arena and px is not None
+    dgamma = dbeta = None
+    if not (acc_inplace or acc_in_exchange):
+        dgamma = torch.empty(C, dtype=torch.float32, device=dsums.device)
+        dbeta = torch.empty(C, dtype=torch.float32, device=dsums.device)
+        call('pxl_bn_bwd_params', _p(dsums), C, _p(dgamma), _p(dbeta), 0, _stream())
+    if group is not None:
+        if px is not None:
+            px.allreduce_bn(dsums, param_grads=(gamma.grad, beta.grad) if acc_in_exchange else None)
+        else:
+            import torch.distributed as dist
+            dist.all_reduce(dsums, group=group)
+    if acc_inplace:
+        return dgamma, dbeta, gamma.grad, beta.grad
+    return dgamma, dbeta, None, None
+
+
 class _BnAct(torch.autograd.Function):
     """_SynchronizedBatchNorm.forward (batchnorm.py:48-78) fused with the ReLU / residual add that
     follow it in Bottleneck.forward (resnet.py:33-48).  ``group``: torch.distributed group whose
@@ -1057,43 +1049,21 @@ class _BnAct(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gamma, beta, running_mean, running_var, residual, training, momentum, eps, relu, group, clamp_var, sums=None):
         _chk(x, 'x', cl=True)
+        if residual is not None:
+            _chk(residual, 'residual', cl=True)
         N, C, H, W = x.shape
         rows = N * H * W
         dev = x.device
         y = torch.empty_like(x)
         coeff = torch.empty((4, C), dtype=torch.float32, device=dev)     # mean, invstd, scale, shift
-        count = float(rows)
-        clamp = 1 if clamp_var else 0
-        applied = False
         if training:
             if sums is None:
                 sums = _stat_zeros(2 * C, dev)
                 call('pxl_bn_stats', _p(x), rows, C, _p(sums), _stream())
-            fused = False
-            if group is not None:
-                import torch.distributed as dist
-                count = float(rows) * dist.get_world_size(group)
-                clamp = 1     # batchnorm.py:125: the multi-replica path clamps var instead of adding eps
-                px = _peer_exchanges.get(id(group))
-                if px is not None and 2 * C <= 4096:
-                    # NVLink peer-memory exchange fused with the finalize (csrc/peer_exchange.cu)
-                    px.allreduce_bn(sums, (count, C, gamma, beta, running_mean, running_var, momentum, eps, clamp,
-                                           coeff[0], coeff[1], coeff[2], coeff[3]))
-                    fused = True
-                else:
-                    dist.all_reduce(sums, group=group)
-            if residual is not None:
-                _chk(residual, 'residual', cl=True)
-            if group is None and FUSE_BN_FINALIZE:
-                # local statistics: finalize + apply in one launch
-                call('pxl_bn_finalize_apply', _p(x), _p(sums), count, _p(gamma), _p(beta), _p(running_mean), _p(running_var),
-                     float(momentum), float(eps), clamp, _p(coeff[0]), _p(coeff[1]), _p(coeff[2]), _p(coeff[3]),
-                     _p(residual), int(relu), _p(y), rows, C, _stream())
-                applied = True
-            elif not fused:
-                call('pxl_bn_finalize', _p(sums), count, C, _p(gamma), _p(beta), _p(running_mean), _p(running_var),
-                     float(momentum), float(eps), clamp, _p(coeff[0]), _p(coeff[1]), _p(coeff[2]), _p(coeff[3]), _stream())
+            count = _bn_train_forward(x, sums, rows, C, gamma, beta, running_mean, running_var, momentum, eps, clamp_var,
+                                      group, coeff, residual, relu, y)
         else:
+            count = float(rows)
             call('pxl_bn_eval_coeffs', C, _p(gamma), _p(beta), _p(running_mean), _p(running_var), float(eps),
                  _p(coeff[2]), _p(coeff[3]), _stream())
             if torch.is_grad_enabled() and (x.requires_grad or gamma.requires_grad):
@@ -1101,9 +1071,6 @@ class _BnAct(torch.autograd.Function):
                 # constants; mean / inv_std slots hold them for bn_bwd_reduce (tiny per-channel torch ops)
                 coeff[0].copy_(running_mean)
                 coeff[1].copy_(torch.rsqrt(running_var + eps))
-        if not applied:
-            if residual is not None:
-                _chk(residual, 'residual', cl=True)
             call('pxl_bn_apply', _p(x), _p(coeff[2]), _p(coeff[3]), _p(residual), int(relu), _p(y), rows, C, _stream())
         ctx.save_for_backward(x, y if (relu and residual is not None) else None, gamma, coeff, running_var, beta)
         ctx.meta = (rows, C, count, bool(relu), residual is not None, bool(training), float(eps), group)
@@ -1116,53 +1083,24 @@ class _BnAct(torch.autograd.Function):
         dy = as_cl(dy)
         dev = dy.device
         dsums = _stat_zeros(2 * C, dev)
-        if not training:
-            # F.batch_norm(training=False) backward: dx = dz * gamma / sqrt(running_var + eps), d(gamma) = sum dz * xhat,
-            # d(beta) = sum dz with xhat from the running statistics.  The reduce launch gives the parameter sums; the
-            # dx launch runs with zero batch sums, which removes its mean terms.
-            ymask = y if (relu and has_res) else None
-            call('pxl_bn_bwd_reduce', _p(x), _p(ymask), _p(dy), _p(coeff[0]), _p(coeff[1]), int(relu), rows, C, _p(dsums),
-                 _p(coeff[2]), _p(coeff[3]), _stream())
-            dgamma = torch.empty(C, dtype=torch.float32, device=dev)
-            dbeta = torch.empty(C, dtype=torch.float32, device=dev)
-            call('pxl_bn_bwd_params', _p(dsums), C, _p(dgamma), _p(dbeta), 0, _stream())
-            zsums = _stat_zeros(2 * C, dev)
-            dx = torch.empty_like(x)
-            dres = torch.empty_like(x) if has_res else None
-            call('pxl_bn_bwd_dx', _p(x), _p(ymask), _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(zsums), count, int(relu),
-                 _p(dx), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]), _p(None), _p(None), _stream())
-            return dx, dgamma, dbeta, None, None, dres, None, None, None, None, None, None, None
         # ReLU without residual: the mask is recomputed from x (same fmaf as the forward) instead of reading y
         ymask = y if (relu and has_res) else None
         call('pxl_bn_bwd_reduce', _p(x), _p(ymask), _p(dy), _p(coeff[0]), _p(coeff[1]), int(relu), rows, C, _p(dsums),
              _p(coeff[2]), _p(coeff[3]), _stream())
-        # single GPU with arena gradients in place: the dx launch adds d(gamma), d(beta) straight into .grad
-        grads_in_arena = (ACCUM_WGRAD_INPLACE and gamma.grad is not None and beta.grad is not None
-                          and gamma.grad.is_contiguous() and beta.grad.is_contiguous())
-        px = _peer_exchanges.get(id(group)) if group is not None else None
-        if px is not None and 2 * C > 4096:
-            px = None
-        # d(gamma), d(beta) come from the LOCAL sums (DDP averages them with the other gradients); whenever the
-        # gradient arena is in place they are accumulated by a launch that runs anyway: the dx kernel (single GPU)
-        # or the peer-exchange kernel (before it exchanges the sums)
-        acc_inplace = grads_in_arena and group is None
-        acc_in_exchange = grads_in_arena and px is not None
-        dgamma = dbeta = None
-        if not (acc_inplace or acc_in_exchange):
+        if not training:
+            # F.batch_norm(training=False) backward: dx = dz * gamma / sqrt(running_var + eps), d(gamma) = sum dz * xhat,
+            # d(beta) = sum dz with xhat from the running statistics.  The reduce launch gives the parameter sums; the
+            # dx launch runs with zero batch sums, which removes its mean terms.
             dgamma = torch.empty(C, dtype=torch.float32, device=dev)
             dbeta = torch.empty(C, dtype=torch.float32, device=dev)
             call('pxl_bn_bwd_params', _p(dsums), C, _p(dgamma), _p(dbeta), 0, _stream())
-        if group is not None:
-            if px is not None:
-                px.allreduce_bn(dsums, param_grads=(gamma.grad, beta.grad) if acc_in_exchange else None)
-            else:
-                import torch.distributed as dist
-                dist.all_reduce(dsums, group=group)
+            dsums, gacc, bacc = _stat_zeros(2 * C, dev), None, None
+        else:
+            dgamma, dbeta, gacc, bacc = _bn_backward_sums(dsums, C, gamma, beta, group)
         dx = torch.empty_like(x)
         dres = torch.empty_like(x) if has_res else None
         call('pxl_bn_bwd_dx', _p(x), _p(ymask), _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, int(relu),
-             _p(dx), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]),
-             _p(gamma.grad if acc_inplace else None), _p(beta.grad if acc_inplace else None), _stream())
+             _p(dx), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc), _stream())
         return dx, dgamma, dbeta, None, None, dres, None, None, None, None, None, None, None
 
 
@@ -1179,56 +1117,13 @@ def bn_act(x, gamma, beta, running_mean, running_var, training=True, momentum=0.
 # conv -> BN -> (+residual) -> (ReLU) as one node on the fp16-pair path
 # ------------------------------------------------------------------------------------------------
 
-# Weight gradients are off the critical path of the backward pass (nothing reads them before the optimiser step), so
-# they could run on a side stream right after the dX pair they consume exists, overlapping the HBM-bound BatchNorm
-# backward launches.  Off by default: the wgrad CTAs (up to ~220 KB of shared memory each) take SMs away from the
-# persistent one-CTA-per-SM convolutions of the critical path, which then wait for them.  Not measured on the H100.
-# Opt-in: PXL_WGRAD_SIDE_STREAM=1.
-# block outputs: ReLU mask for the backward as 1 byte per 4 values (A/B switch; 0 re-reads the fp32 result)
-BN_RELU_MASK = _os.environ.get('PXL_BN_RELU_MASK', '1') != '0'
-WGRAD_SIDE_STREAM = _os.environ.get('PXL_WGRAD_SIDE_STREAM', '0') != '0'
-_side_streams = {}
-
-
-def _wgrad_stream(device):
-    s = _side_streams.get(device)
-    if s is None:
-        s = _side_streams[device] = [torch.cuda.Stream(device=device), False, False]
-    return s
-
-
-def _join_after_backward():
-    for ent in _side_streams.values():
-        ent[2] = False
-    join_side_streams()
-
-
-def join_side_streams():
-    """Make the current stream wait for every side-stream launch so far (called before gradients are consumed:
-    all-reduce, optimiser step, zero_grad)."""
-    for ent in _side_streams.values():
-        if ent[1]:
-            torch.cuda.current_stream().wait_stream(ent[0])
-            ent[1] = False
-
-
 _residual_stash = {}            # block key -> gradient of the residual branch waiting for the block's first dgrad (one step)
 H16_DX_TARGET_LOG2 = 12         # bn_bwd_dx: max|gamma*invstd| * absmax(dz) -> <= 2^12, 3 bits of headroom for the mean terms
 _unit_out_pair = None           # H16 of the last _ConvBnAct.forward output (picked up by conv_bn_act right after apply)
 
 
-def _pair_of(x, want_lo):
-    """The fp16 pair of an activation: attached by its producer (same step, unmodified), else split now (cached)."""
-    ent = getattr(x, '_pxl_h16', None)
-    if ent is not None and ent[0] == _epoch and ent[1] == x._version and ent[2] == x.data_ptr() and ent[3].has_lo >= want_lo:
-        return ent[3]
-    if getattr(x, '_pxl_carrier', False):
-        raise RuntimeError('fp16-pair carrier tensor without a valid pair (stale step?)')
-    return h16_cached(x, H16_ACT_SCALE, want_lo)
-
-
 def _attach_pair(t, h, carrier=False):
-    t._pxl_h16 = (_epoch, t._version, t.data_ptr(), h)
+    _step_put(t, '_pxl_h16', h)
     if carrier:
         t._pxl_carrier = True
     return t
@@ -1262,17 +1157,13 @@ class _ConvBnAct(torch.autograd.Function):
         Cout, Cin2, kh, kw = weight.shape
         if Cin2 != Cin:
             raise ValueError('channel mismatch')
-        OH = (H + 2 * padding - dilation * (kh - 1) - 1) // stride + 1
-        OW = (W + 2 * padding - dilation * (kw - 1) - 1) // stride + 1
-        taps = _taps(kh, kw, dilation, padding)
+        OH, OW, taps = _conv_geometry(H, W, kh, kw, stride, padding, dilation)
         xh = _pair_of(x, want_lo)
         dev = xh.device
         sums = _stat_zeros(2 * Cout, dev)
         c = conv_raw(xh, weight, None, taps, N, H, W, Cin, OH, OW, Cout, Cout, stride, 1, bn_stats=sums)
         rows = N * OH * OW
         n = rows * Cout
-        count = float(rows)
-        clamp = 1 if clamp_var else 0
         coeff = torch.empty((4, Cout), dtype=torch.float32, device=dev)
         pair = torch.empty((2, n), dtype=torch.float16, device=dev) if out_mode != 'fp32' else None
         y = torch.empty_like(c) if out_mode != 'pair' else None
@@ -1281,34 +1172,12 @@ class _ConvBnAct(torch.autograd.Function):
         # block output (residual + ReLU): the backward takes the ReLU mask from one byte per 4 values instead of
         # re-reading the fp32 result in both of its launches
         mask = (torch.empty(n // 4, dtype=torch.uint8, device=dev)
-                if (BN_RELU_MASK and relu and residual is not None and any(ctx.needs_input_grad)) else None)
+                if (relu and residual is not None and any(ctx.needs_input_grad)) else None)
         if residual is not None:
             _chk(residual, 'residual', cl=True)
-        applied = fused = False
-        if group is not None:
-            import torch.distributed as dist
-            count = float(rows) * dist.get_world_size(group)
-            clamp = 1     # batchnorm.py:125: the multi-replica path clamps var instead of adding eps
-            px = _peer_exchanges.get(id(group))
-            if px is not None and 2 * Cout <= 4096:
-                px.allreduce_bn(sums, (count, Cout, gamma, beta, running_mean, running_var, momentum, eps, clamp,
-                                       coeff[0], coeff[1], coeff[2], coeff[3]))
-                fused = True
-            else:
-                dist.all_reduce(sums, group=group)
-        if group is None and FUSE_BN_FINALIZE:
-            call('pxl_bn_finalize_apply_h16', _p(c), _p(sums), count, _p(gamma), _p(beta), _p(running_mean), _p(running_var),
-                 float(momentum), float(eps), clamp, _p(coeff[0]), _p(coeff[1]), _p(coeff[2]), _p(coeff[3]),
-                 _p(residual), int(relu), _p(y), rows, Cout, _p(hi), _p(lo), float(H16_ACT_SCALE), _p(mask), _stream())
-            applied = True
-        elif not fused:
-            call('pxl_bn_finalize', _p(sums), count, Cout, _p(gamma), _p(beta), _p(running_mean), _p(running_var),
-                 float(momentum), float(eps), clamp, _p(coeff[0]), _p(coeff[1]), _p(coeff[2]), _p(coeff[3]), _stream())
-        if not applied:
-            call('pxl_bn_apply_h16', _p(c), _p(coeff[2]), _p(coeff[3]), _p(residual), int(relu), _p(y), rows, Cout,
-                 _p(hi), _p(lo), float(H16_ACT_SCALE), _p(mask), _stream())
-        ctx.save_for_backward(xh.buf, weight, c, mask if BN_RELU_MASK else (y if (relu and residual is not None) else None),
-                              gamma, coeff, beta)
+        count = _bn_train_forward(c, sums, rows, Cout, gamma, beta, running_mean, running_var, momentum, eps, clamp_var,
+                                  group, coeff, residual, relu, y, (_p(hi), _p(lo), float(H16_ACT_SCALE), _p(mask)))
+        ctx.save_for_backward(xh.buf, weight, c, mask, gamma, coeff, beta)
         ctx.meta = (taps, N, H, W, Cin, OH, OW, Cout, stride, kh * kw, count, bool(relu), residual is not None, group,
                     xh.scale, want_lo, prec)
         _unit_out_pair = H16(pair, n, H16_ACT_SCALE, None, want_lo) if pair is not None else None
@@ -1331,34 +1200,13 @@ class _ConvBnAct(torch.autograd.Function):
         slot = _scale_slot(dev)
         if relu and has_res and mask is None:
             raise RuntimeError('the ReLU mask of a residual unit was not recorded in the forward')
-        ymask = None
-        if mask is not None and mask.dtype != torch.uint8:      # PXL_BN_RELU_MASK=0: the fp32 result is the mask
-            ymask, mask = mask, None
-        call('pxl_bn_bwd_reduce_h16', _p(c), _p(ymask), _p(dy), _p(coeff[0]), _p(coeff[1]), int(relu), rows, C, _p(dsums),
+        call('pxl_bn_bwd_reduce_h16', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), int(relu), rows, C, _p(dsums),
              _p(coeff[2]), _p(coeff[3]), _p(slot), _p(mask), _stream())
-        grads_in_arena = (ACCUM_WGRAD_INPLACE and gamma.grad is not None and beta.grad is not None
-                          and gamma.grad.is_contiguous() and beta.grad.is_contiguous())
-        px = _peer_exchanges.get(id(group)) if group is not None else None
-        if px is not None and 2 * C > 4096:
-            px = None
-        acc_inplace = grads_in_arena and group is None
-        acc_in_exchange = grads_in_arena and px is not None
-        dgamma = dbeta = None
-        if not (acc_inplace or acc_in_exchange):
-            dgamma = torch.empty(C, dtype=torch.float32, device=dev)
-            dbeta = torch.empty(C, dtype=torch.float32, device=dev)
-            call('pxl_bn_bwd_params', _p(dsums), C, _p(dgamma), _p(dbeta), 0, _stream())
-        if group is not None:
-            if px is not None:
-                px.allreduce_bn(dsums, param_grads=(gamma.grad, beta.grad) if acc_in_exchange else None)
-            else:
-                import torch.distributed as dist
-                dist.all_reduce(dsums, group=group)
+        dgamma, dbeta, gacc, bacc = _bn_backward_sums(dsums, C, gamma, beta, group)
         dpair = torch.empty((2, n), dtype=torch.float16, device=dev)
         dres = torch.empty_like(c) if has_res else None
-        call('pxl_bn_bwd_dx_h16', _p(c), _p(ymask), _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, int(relu),
-             _p(None), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]),
-             _p(gamma.grad if acc_inplace else None), _p(beta.grad if acc_inplace else None),
+        call('pxl_bn_bwd_dx_h16', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, int(relu),
+             _p(None), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc),
              _p(dpair[0]), _p(dpair[1] if want_lo else None), _p(slot), H16_DX_TARGET_LOG2, _p(mask), _stream())
         dh = H16(dpair, n, None, slot, want_lo)
         dx = dw = None
@@ -1370,12 +1218,7 @@ class _ConvBnAct(torch.autograd.Function):
             dres = None
         give_dx = stash_role == 'give_dx' and _residual_stash.get(stash_key) is None
         if ctx.needs_input_grad[0]:
-            arena, off = _arena_of(weight) if BATCH_WEIGHT_PREP else (None, None)
-            if arena is not None and arena._conv_at.get(off) == (Cout, T, Cin):
-                nw = weight.numel()
-                wt = H16(arena.derived('h16_t')[:, off:off + nw], nw, H16_W_SCALE, None, True)
-            else:
-                wt = h16_split(transpose_weights(weight, Cout, T, Cin), H16_W_SCALE, want_lo)
+            wt = conv_weight(weight, 'h16', (Cout, T, Cin), transposed=True, want_lo=want_lo)
             held = _residual_stash.pop(stash_key, None) if stash_role == 'take' else None
             if stash_role == 'take' and held is None:
                 _residual_stash[stash_key] = 'taken'          # a 'give_dx' unit that runs later returns its dX itself
@@ -1398,35 +1241,19 @@ class _ConvBnAct(torch.autograd.Function):
             _residual_stash[stash_key] = dx
             dx = None
         if ctx.needs_input_grad[1]:
-            inplace = ACCUM_WGRAD_INPLACE and weight.grad is not None and weight.grad.is_contiguous(memory_format=CL)
+            inplace = weight.grad is not None and weight.grad.is_contiguous(memory_format=CL)
             dwbuf = weight.grad if inplace else torch.zeros_like(weight, memory_format=torch.preserve_format)
-            xh = H16(xbuf, xbuf.shape[1], xscale, None, want_lo)
-            if WGRAD_SIDE_STREAM and inplace:
-                ent = _wgrad_stream(dev)
-                main = torch.cuda.current_stream()
-                ev = torch.cuda.Event()
-                ev.record(main)                         # the dX pair (and everything before it) is enqueued
-                ent[0].wait_event(ev)
-                with torch.cuda.stream(ent[0]):
-                    conv_wgrad_raw(xh, dh, dwbuf, taps, N, H, W, Cin, OH, OW, Cout, Cout, stride, 1, precision=prec)
-                dpair.record_stream(ent[0])
-                xbuf.record_stream(ent[0])
-                ent[1] = True
-                if not ent[2]:
-                    # whoever reads .grad after loss.backward() does so on the main stream: join when this backward ends
-                    ent[2] = True
-                    torch.autograd.Variable._execution_engine.queue_callback(_join_after_backward)
-            else:
-                conv_wgrad_raw(xh, dh, dwbuf, taps, N, H, W, Cin, OH, OW, Cout, Cout, stride, 1, precision=prec)
+            conv_wgrad_raw(H16(xbuf, xbuf.shape[1], xscale, None, want_lo), dh, dwbuf, taps, N, H, W, Cin, OH, OW, Cout, Cout,
+                           stride, 1, precision=prec)
             dw = None if inplace else dwbuf
         return (dx, dw, dgamma, dbeta, None, None, dres) + (None,) * 11
 
 
 def conv_bn_unit_ok(conv, bn):
-    """True when conv -> bn can run as one _ConvBnAct node: fp16-pair precision, train-mode BN, bias-free conv with
-    64-aligned channel counts and stride 1 / 2."""
-    return (_conv_precision >= 3 and bn.training and conv.bias is None and not conv.out_lanes
-            and conv.in_channels % 64 == 0 and conv.out_channels % 64 == 0 and conv.stride in (1, 2))
+    """True when conv -> bn can run as one _ConvBnAct node: train-mode BN, a bias-free convolution without padded output
+    lanes, and the fp16-pair kernels serving its forward, dgrad and wgrad (the wgrad's rule implies the other two)."""
+    return (bn.training and conv.bias is None and not conv.out_lanes
+            and conv_route('wgrad', conv.in_channels, conv.out_channels, conv.stride, 1, _conv_precision)[0] == 'h16')
 
 
 def conv_bn_act(x, conv, bn, relu=False, residual=None, out_mode='both', stash_key=None, stash_role=None):

@@ -116,7 +116,7 @@ def device_prefetch(data_loader):
         return
     # the copy stream, the staging slots and their "consumed" events live as long as the process: a new side stream per
     # epoch gets no cached blocks from torch's (per-stream) allocator pools, and a cudaMalloc of the 67 MB slots at the
-    # start of an epoch stalls the step (tools/e2e_probe2.py)
+    # start of an epoch stalls the step
     state = _prefetch_state.get(torch.cuda.current_device())
     if state is None:
         state = _prefetch_state[torch.cuda.current_device()] = {
