@@ -61,6 +61,21 @@ int pxl_ce2d(const float* logits, const float* labels, int n, int C, int64_t HW,
              void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Cross Pseudo Supervision (Chen et al., CVPR 2021): cross-entropy of each student's logits
+ * against the per-pixel argmax of the other side's pseudo-label source.  All maps planar
+ * [n, C, H*W]; t_l / t_r may be the same pointers as s_l / s_r (plain CPS: 16*C B/pixel) or
+ * separate maps (CutMix CPS: 24*C B/pixel).  argmax takes the first maximal index.
+ *   per_sample[b]     = mean_p (logsumexp(s_l[b,:,p]) - s_l[b, argmax_c t_r[b,c,p], p])
+ *   per_sample[n + b] = the same with l and r swapped
+ *   grad_l = grad_scale/HW * (softmax(s_l) - onehot(argmax t_r)), grad_r symmetrically;
+ *   both NULL (loss only) or both set.  C <= 32 (else PXL_ERR_UNSUPPORTED).  Sums are taken in a
+ *   fixed order: repeated calls are bit-identical.
+ * ------------------------------------------------------------------------------------------- */
+int pxl_cps_ce(const float* s_l, const float* s_r, const float* t_l, const float* t_r,
+               int n, int C, int64_t HW, float grad_scale, float* per_sample,
+               float* grad_l, float* grad_r, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Channel softmax on planar maps: F.softmax(pred, dim=1), task/sseg/model.py:62,121;
  * task/sseg/func.py:216-220
  * ------------------------------------------------------------------------------------------- */

@@ -9,21 +9,29 @@ Importing the package does not need a GPU; the first kernel call loads lib/libpi
 from .version import __version__
 from .utils import log_info, log_warn, log_err, str2bool, str2intlist, REGRESSION, CLASSIFICATION
 from . import nn, ssl_algorithm
-from .ssl_algorithm import SSL_NULL, SSL_MT, SSL_ADV, SSL_S4L, SSL_GCT, SSL_CCT, SSL_CUTMIX, SSL_ALGORITHMS
+from .ssl_algorithm import (SSL_NULL, SSL_MT, SSL_ADV, SSL_S4L, SSL_GCT, SSL_CCT, SSL_CUTMIX, SSL_CPS,
+                            SSL_ALGORITHMS)
 from .runner import create_parser, build_args, run_script
 
 
 def register_into_pixelssl(pixelssl_module=None, task_sseg_modules=None):
     """Drop the engine in under an unmodified ``pixelssl.runner`` / ``TaskProxy``: replaces the
-    algorithm modules TaskProxy looks up by name (task_template/proxy.py:433-434) and, if the
-    task's ``model`` / ``criterion`` modules are given, their export functions
-    (proxy.py:426-427)."""
+    algorithm modules TaskProxy looks up by name (task_template/proxy.py:433-434), adds the ones
+    PixelSSL does not have (``ssl_cps``) to ``pixelssl.ssl_algorithm.SSL_ALGORITHMS`` (the list
+    ``pixelssl.runner.create_parser`` checks names against) and, if the task's ``model`` /
+    ``criterion`` modules are given, replaces their export functions (proxy.py:426-427)."""
     if pixelssl_module is None:
         import pixelssl as pixelssl_module
+    names = getattr(pixelssl_module.ssl_algorithm, 'SSL_ALGORITHMS', None)
+    if names is None:
+        names = []
+        pixelssl_module.ssl_algorithm.SSL_ALGORITHMS = names
     for name in SSL_ALGORITHMS:
         mod = getattr(ssl_algorithm, name)
         pixelssl_module.ssl_algorithm.__dict__[name] = mod
         setattr(pixelssl_module.ssl_algorithm, name, mod)
+        if name not in names:
+            names.append(name)
     # the proxy builds its sampler through ``pixelssl.nn.data`` by attribute (task_template/proxy.py:11,372):
     # the rank-aware sampler has the same constructor and, at world size 1, the same index stream
     from .nn import data as b200_data

@@ -36,6 +36,7 @@ SIGNATURES = {
     'pxl_mse_consistency': (c_int, [P, P, c_int64, c_float, P, P, P, P]),
     'pxl_mse_consistency_bwd': (c_int, [P, P, c_int64, c_float, P, P, P]),
     'pxl_ce2d': (c_int, [P, P, c_int, c_int, c_int64, c_int, P, P, P, c_float, P]),
+    'pxl_cps_ce': (c_int, [P, P, P, P, c_int, c_int, c_int64, c_float, P, P, P, P]),
     'pxl_softmax_planar': (c_int, [P, P, c_int, c_int, c_int64, P]),
     'pxl_softmax_planar_bwd': (c_int, [P, P, P, c_int, c_int, c_int64, P]),
     'pxl_softmax_mse': (c_int, [P, P, c_int, c_int, c_int64, c_float, P, P, P, P, P]),

@@ -1,5 +1,6 @@
 // Pixel-wise loss kernels on planar [n, C, H*W] maps: MSE consistency (the metric kernel),
-// cross-entropy with ignore_index, channel softmax, fused softmax+MSE, CutMix mix/confidence.
+// cross-entropy with ignore_index, the cross-pseudo-label (CPS) cross-entropy, channel softmax,
+// fused softmax+MSE, CutMix mix/confidence.
 #include "common.cuh"
 #include <stdlib.h>
 #include <math_constants.h>
@@ -266,6 +267,144 @@ extern "C" int pxl_ce2d(const float* logits, const float* labels, int n, int C, 
     else ce2d_kernel<false><<<grid, 256, 0, st>>>(logits, labels, C, HW, ignore_index, part, nullptr, nullptr, 0.f);
     PXL_CHECK_LAUNCH();
     ce2d_sum_kernel<<<(unsigned)pxl_cdiv(n, 128), 128, 0, st>>>(part, (int)grid.x, n, per_sample);
+    PXL_CHECK_LAUNCH();
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// Cross Pseudo Supervision loss (Chen et al., CVPR 2021): each of two students is trained with
+// cross-entropy against the per-pixel argmax of the other's map.  One thread per pixel, the C
+// channel planes read coalesced as in ce2d_kernel; both students' logits stay in registers.
+//   per_sample[b]     = mean_p (logsumexp(s_l[b,:,p]) - s_l[b, argmax_c t_r[b,c,p], p])
+//   per_sample[n + b] = the same with l and r swapped
+//   grad_x            = grad_scale / HW * (softmax(s_x) - onehot(pseudo-label of x))
+// argmax takes the first maximal index (torch's rule; a NaN counts as the maximum, as in torch).
+//   algorithmic traffic: aliased targets (t_l == s_l, t_r == s_r): read s_l, s_r + write grad_l,
+//   grad_r = 16*C B/pixel; separate targets: + read t_l, t_r = 24*C B/pixel.  Without gradients
+//   8*C and 16*C B/pixel.
+// fp64 per-block partials, summed in a fixed order by cps_sum_kernel: no atomics, so repeated calls
+// are bit-identical.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool cps_beats(float v, float best) { return v > best || (v != v && best == best); }
+
+__device__ __forceinline__ int cps_argmax_planes(const float* __restrict__ t, int C, int64_t HW) {
+    int y = 0;
+    float best = t[0];
+#pragma unroll
+    for (int c = 1; c < CE_MAXC; ++c)
+        if (c < C) {
+            const float v = t[(int64_t)c * HW];
+            if (cps_beats(v, best)) { best = v; y = c; }
+        }
+    return y;
+}
+
+// cross-entropy of one pixel's logits v against label y; v is overwritten with exp(v - max)
+template <bool WRITE_GRAD>
+__device__ __forceinline__ float cps_pixel(float (&v)[CE_MAXC], int C, int y, float g, float* __restrict__ gp,
+                                           int64_t HW) {
+    float m = -CUDART_INF_F;
+#pragma unroll
+    for (int c = 0; c < CE_MAXC; ++c)
+        if (c < C) m = fmaxf(m, v[c]);
+    float se = 0.f, x_y = 0.f;
+#pragma unroll
+    for (int c = 0; c < CE_MAXC; ++c)
+        if (c < C) {
+            if (c == y) x_y = v[c];      // select in the unrolled loop: no dynamic register indexing
+            v[c] = expf(v[c] - m);
+            se += v[c];
+        }
+    if (WRITE_GRAD) {
+        const float inv = g / se;
+#pragma unroll
+        for (int c = 0; c < CE_MAXC; ++c)
+            if (c < C) {
+                float gv = v[c] * inv;
+                if (c == y) gv -= g;
+                gp[(int64_t)c * HW] = gv;
+            }
+    }
+    return (logf(se) + m) - x_y;
+}
+
+template <bool ALIAS, bool WRITE_GRAD>
+__global__ void __launch_bounds__(256)
+cps_ce_kernel(const float* __restrict__ s_l, const float* __restrict__ s_r, const float* __restrict__ t_l,
+              const float* __restrict__ t_r, int n, int C, int64_t HW, float g, double* __restrict__ part,
+              float* __restrict__ grad_l, float* __restrict__ grad_r) {
+    const int b = blockIdx.y;
+    const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    double loss_l = 0.0, loss_r = 0.0;
+    if (p < HW) {
+        const int64_t base = (int64_t)b * C * HW + p;
+        // y_l: argmax of t_l, the label r learns from; y_r: argmax of t_r, the label l learns from.  Aliased targets
+        // take the argmax while the logits load (a separate pass over the registers spills in the loss-only variant).
+        int y_l = 0, y_r = 0;
+        if (!ALIAS) { y_l = cps_argmax_planes(t_l + base, C, HW); y_r = cps_argmax_planes(t_r + base, C, HW); }
+        float vl[CE_MAXC], vr[CE_MAXC];
+        float bl = 0.f, br = 0.f;
+#pragma unroll
+        for (int c = 0; c < CE_MAXC; ++c)
+            if (c < C) {
+                vl[c] = s_l[base + (int64_t)c * HW];
+                vr[c] = s_r[base + (int64_t)c * HW];
+                if (ALIAS) {
+                    if (c == 0 || cps_beats(vl[c], bl)) { bl = vl[c]; y_l = c; }
+                    if (c == 0 || cps_beats(vr[c], br)) { br = vr[c]; y_r = c; }
+                }
+            }
+        loss_l = (double)cps_pixel<WRITE_GRAD>(vl, C, y_r, g, WRITE_GRAD ? grad_l + base : nullptr, HW);
+        loss_r = (double)cps_pixel<WRITE_GRAD>(vr, C, y_l, g, WRITE_GRAD ? grad_r + base : nullptr, HW);
+    }
+    __shared__ double wp[2][8];
+    loss_l = warp_sum_d(loss_l);
+    loss_r = warp_sum_d(loss_r);
+    if ((threadIdx.x & 31) == 0) { wp[0][threadIdx.x >> 5] = loss_l; wp[1][threadIdx.x >> 5] = loss_r; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double sl = 0.0, sr = 0.0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { sl += wp[0][i]; sr += wp[1][i]; }
+        part[(int64_t)b * gridDim.x + blockIdx.x] = sl;
+        part[(int64_t)(n + b) * gridDim.x + blockIdx.x] = sr;
+    }
+}
+
+// per_sample[i] = (sum of row i's partials) / HW, i < 2n.  One warp per row: lane j adds partials j, j+32, ... in
+// order, then a fixed shuffle tree - the same order on every call, and 32 loads in flight instead of one chain.
+#define CPS_SUM_ROWS 4
+__global__ void __launch_bounds__(32 * CPS_SUM_ROWS)
+cps_sum_kernel(const double* __restrict__ part, int nblk, int rows, double inv_hw, float* __restrict__ per_sample) {
+    const int i = blockIdx.x * CPS_SUM_ROWS + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (i >= rows) return;                      // warp-uniform
+    double s = 0.0;
+    for (int k = lane; k < nblk; k += 32) s += __ldg(part + (int64_t)i * nblk + k);
+    s = warp_sum_d(s);
+    if (lane == 0) per_sample[i] = (float)(s * inv_hw);
+}
+
+extern "C" int pxl_cps_ce(const float* s_l, const float* s_r, const float* t_l, const float* t_r,
+                          int n, int C, int64_t HW, float grad_scale, float* per_sample,
+                          float* grad_l, float* grad_r, void* stream) {
+    if (!s_l || !s_r || !t_l || !t_r || !per_sample || n <= 0 || C <= 0 || HW <= 0) return PXL_ERR_BAD_ARG;
+    if ((grad_l == nullptr) != (grad_r == nullptr)) return PXL_ERR_BAD_ARG;
+    if (C > CE_MAXC || n > 65535) return PXL_ERR_UNSUPPORTED;
+    cudaStream_t st = (cudaStream_t)stream;
+    dim3 grid((unsigned)pxl_cdiv(HW, 256), (unsigned)n);
+    int rc = 0;
+    double* part = (double*)pxl_workspace_(PXL_WS_CPS, stream, (size_t)grid.x * 2 * n * sizeof(double), &rc);
+    if (rc) return rc;
+    const bool alias = (t_l == s_l) && (t_r == s_r);
+    const float g = (float)((double)grad_scale / (double)HW);
+    if (alias && grad_l) cps_ce_kernel<true, true><<<grid, 256, 0, st>>>(s_l, s_r, nullptr, nullptr, n, C, HW, g, part, grad_l, grad_r);
+    else if (alias) cps_ce_kernel<true, false><<<grid, 256, 0, st>>>(s_l, s_r, nullptr, nullptr, n, C, HW, g, part, nullptr, nullptr);
+    else if (grad_l) cps_ce_kernel<false, true><<<grid, 256, 0, st>>>(s_l, s_r, t_l, t_r, n, C, HW, g, part, grad_l, grad_r);
+    else cps_ce_kernel<false, false><<<grid, 256, 0, st>>>(s_l, s_r, t_l, t_r, n, C, HW, g, part, nullptr, nullptr);
+    PXL_CHECK_LAUNCH();
+    cps_sum_kernel<<<(unsigned)pxl_cdiv(2 * n, CPS_SUM_ROWS), 32 * CPS_SUM_ROWS, 0, st>>>(part, (int)grid.x, 2 * n,
+                                                                                       1.0 / (double)HW, per_sample);
     PXL_CHECK_LAUNCH();
     return 0;
 }

@@ -212,6 +212,65 @@ def cross_entropy2d(logits, gt, ignore_index=255, upstream_const=None):
     return _CrossEntropy2d.apply(logits.contiguous(), gt.contiguous(), ignore_index, upstream_const)
 
 
+def cps_raw(s_l, s_r, t_l, t_r, grad_scale, want_grad):
+    """One pxl_cps_ce launch.  Returns (per_sample[2n]: l rows then r rows, grad_l or None, grad_r or None).
+    The timer metadata of the launch is its algorithmic traffic in bytes: the two student maps, the two target maps
+    unless they are the students', the two gradients if written."""
+    n, c, h, w = s_l.shape
+    per = torch.empty(2 * n, dtype=torch.float32, device=s_l.device)
+    gl = torch.empty_like(s_l) if want_grad else None
+    gr = torch.empty_like(s_r) if want_grad else None
+    aliased = t_l.data_ptr() == s_l.data_ptr() and t_r.data_ptr() == s_r.data_ptr()
+    maps = 2 + (0 if aliased else 2) + (2 if want_grad else 0)
+    _timed_call('pxl_cps_ce', _p(s_l), _p(s_r), _p(t_l), _p(t_r), n, c, h * w, float(grad_scale), _p(per), _p(gl), _p(gr),
+                _stream(), meta=4 * maps * s_l.numel())
+    return per, gl, gr
+
+
+class _CpsCrossEntropy(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, s_l, s_r, t_l, t_r, loss_scale, unit_upstream):
+        n = s_l.shape[0]
+        need = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+        fused = need and unit_upstream
+        per, gl, gr = cps_raw(s_l, s_r, t_l, t_r, loss_scale / n, fused)
+        ctx.fused, ctx.scale = fused, loss_scale
+        if need:
+            if fused:
+                ctx.save_for_backward(gl, gr)
+            else:
+                ctx.save_for_backward(s_l, s_r, t_l, t_r)
+        return torch.mean(per[:n]) * loss_scale, torch.mean(per[n:]) * loss_scale
+
+    @staticmethod
+    def backward(ctx, g_l, g_r):
+        if ctx.fused:
+            gl, gr = ctx.saved_tensors
+            return gl, gr, None, None, None, None
+        s_l, s_r, t_l, t_r = ctx.saved_tensors
+        _, gl, gr = cps_raw(s_l, s_r, t_l, t_r, ctx.scale / s_l.shape[0], True)
+        return gl.mul_(g_l), gr.mul_(g_r), None, None, None, None
+
+
+def cps_cross_entropy(s_l, s_r, t_l=None, t_r=None, loss_scale=1.0, unit_upstream=False):
+    """Cross Pseudo Supervision (Chen et al., CVPR 2021) -> (loss_l, loss_r), two 0-d tensors:
+    loss_l = loss_scale * F.cross_entropy(s_l, t_r.argmax(1)), loss_r = loss_scale * F.cross_entropy(s_r, t_l.argmax(1)).
+
+    s_l, s_r: the two students' logits, planar [n,C,H,W].  t_l, t_r: the maps the pseudo-labels are taken from
+    (default: s_l and s_r themselves); they are never differentiated.  argmax takes the first maximal index, as torch's.
+    unit_upstream=True: the caller guarantees that both results are added, un-scaled, into the loss on which
+    ``backward()`` is called, so both gradients are written by the forward launch (16*C B/pixel with aliased targets
+    instead of 8*C + 24*C).  Otherwise backward launches the kernel again and scales by the upstream gradients."""
+    t_l = s_l.detach() if t_l is None else t_l.detach()
+    t_r = s_r.detach() if t_r is None else t_r.detach()
+    for t, name in ((s_l, 's_l'), (s_r, 's_r'), (t_l, 't_l'), (t_r, 't_r')):
+        _chk(t, name)
+        if t.dim() != 4 or t.shape != s_l.shape:
+            raise ValueError('%s: expected a planar [n,C,H,W] map of shape %s, got %s' % (name, tuple(s_l.shape),
+                                                                                          tuple(t.shape)))
+    return _CpsCrossEntropy.apply(s_l, s_r, t_l, t_r, float(loss_scale), bool(unit_upstream))
+
+
 class _Softmax(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits):

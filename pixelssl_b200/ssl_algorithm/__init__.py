@@ -1,5 +1,6 @@
-"""Algorithm registry with the reference's names (pixelssl/ssl_algorithm/__init__.py:10-27)."""
-from . import ssl_base, ssl_null, ssl_mt, ssl_cutmix, ssl_adv, ssl_gct, ssl_cct, ssl_s4l
+"""Algorithm registry with the reference's names (pixelssl/ssl_algorithm/__init__.py:10-27), plus Cross Pseudo
+Supervision (``ssl_cps``), which the reference does not have."""
+from . import ssl_base, ssl_null, ssl_mt, ssl_cutmix, ssl_adv, ssl_gct, ssl_cct, ssl_s4l, ssl_cps
 
 SSL_NULL = ssl_null.SSLNULL.NAME
 SSL_MT = ssl_mt.SSLMT.NAME
@@ -8,5 +9,6 @@ SSL_ADV = ssl_adv.SSLADV.NAME
 SSL_GCT = ssl_gct.SSLGCT.NAME
 SSL_CCT = ssl_cct.SSLCCT.NAME
 SSL_S4L = ssl_s4l.SSLS4L.NAME
+SSL_CPS = ssl_cps.SSLCPS.NAME
 
-SSL_ALGORITHMS = [SSL_NULL, SSL_MT, SSL_ADV, SSL_S4L, SSL_GCT, SSL_CCT, SSL_CUTMIX]
+SSL_ALGORITHMS = [SSL_NULL, SSL_MT, SSL_ADV, SSL_S4L, SSL_GCT, SSL_CCT, SSL_CUTMIX, SSL_CPS]

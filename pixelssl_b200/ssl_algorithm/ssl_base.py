@@ -173,6 +173,26 @@ def to_device(tensors, non_blocking=True):
     return tuple(t.cuda(non_blocking=non_blocking) for t in tensors)
 
 
+def pair_picker(name, model_dict, optimizer_dict, lrer_dict, criterion_dict):
+    """The element dicts of an algorithm that trains two task models side by side (ssl_gct.py:31-48): one entry
+    ``model`` serves both sides, or two entries ``lmodel`` / ``rmodel``.  Returns ``pick(d) -> [left, right]``."""
+    tag = name.upper()
+    if not len(model_dict) == len(optimizer_dict) == len(lrer_dict) == len(criterion_dict):
+        logger.log_err('The len(element_dict) of {0} should be the same\n'.format(tag))
+    if len(model_dict) == 1:
+        if list(model_dict.keys())[0] != 'model':
+            logger.log_err('In {0}, the key of 1-value element_dict should be \'model\',\n'
+                           'but \'{1}\' is given\n'.format(tag, model_dict.keys()))
+        return lambda d: [d['model'], d['model']]
+    if len(model_dict) == 2:
+        if 'lmodel' not in model_dict or 'rmodel' not in model_dict:
+            logger.log_err('In {0}, the key of 2-value element_dict should be \'(lmodel, rmodel)\', '
+                           'but \'{1}\' is given\n'.format(tag, model_dict.keys()))
+        return lambda d: [d['lmodel'], d['rmodel']]
+    logger.log_err('The {0} algorithm supports element_dict with 1 or 2 elements, '
+                   'but given {1} elements\n'.format(tag, len(model_dict)))
+
+
 def check_single_model_dicts(name, model_dict, optimizer_dict, lrer_dict, criterion_dict):
     if not len(model_dict) == len(optimizer_dict) == len(lrer_dict) == len(criterion_dict) == 1:
         logger.log_err('The len(element_dict) of {0} should be 1\n'.format(name.upper()))

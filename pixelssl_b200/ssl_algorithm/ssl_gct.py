@@ -38,21 +38,7 @@ def add_parser_arguments(parser):
 
 
 def ssl_gct(args, model_dict, optimizer_dict, lrer_dict, criterion_dict, task_func):
-    if not len(model_dict) == len(optimizer_dict) == len(lrer_dict) == len(criterion_dict):
-        logger.log_err('The len(element_dict) of SSL_GCT should be the same\n')
-    if len(model_dict) == 1:
-        if list(model_dict.keys())[0] != 'model':
-            logger.log_err('In SSL_GCT, the key of 1-value element_dict should be \'model\',\n'
-                           'but \'{0}\' is given\n'.format(model_dict.keys()))
-        pick = lambda d: [d['model'], d['model']]
-    elif len(model_dict) == 2:
-        if 'lmodel' not in model_dict or 'rmodel' not in model_dict:
-            logger.log_err('In SSL_GCT, the key of 2-value element_dict should be \'(lmodel, rmodel)\', '
-                           'but \'{0}\' is given\n'.format(model_dict.keys()))
-        pick = lambda d: [d['lmodel'], d['rmodel']]
-    else:
-        logger.log_err('The SSL_GCT algorithm supports element_dict with 1 or 2 elements, '
-                       'but given {0} elements\n'.format(len(model_dict)))
+    pick = ssl_base.pair_picker(SSLGCT.NAME, model_dict, optimizer_dict, lrer_dict, criterion_dict)
     algorithm = SSLGCT(args)
     algorithm.build(pick(model_dict), pick(optimizer_dict), pick(lrer_dict), pick(criterion_dict), task_func)
     return algorithm
