@@ -17,10 +17,11 @@
 //   the consumer warpgroups, "a_inkernel").
 // * warp roles: warpgroup 0 = TMA producer (one warp, TMA under elect.sync), warpgroups 1 and 2 = consumers, each
 //   owning 64 of the 128 tile rows (wgmma M = 64).  mbarrier full/empty ring.
-// * accumulation: the tensor core's own fp32 accumulation truncates (its error grows with the number of MMAs summed),
-//   so the MMAs of a stage go into fresh register tiles - the large hi*hi products in two halves of the K slice, the
-//   small lo*hi + hi*lo corrections in a tile of their own - which are added to the running sum with IEEE
-//   round-to-nearest adds.
+// * accumulation: the tensor core's own fp32 accumulation truncates (its error grows with the number of MMAs summed
+//   into one accumulator), so the MMAs of a stage go into fresh register tiles - the large hi*hi products in two halves
+//   of the K slice, the small lo*hi + hi*lo corrections in a tile of their own - which are added to the running sum
+//   with IEEE round-to-nearest adds.  The fp16 loops wait for a group only where an add needs it (schedule at the
+//   consumer loop): the chains and the adds, and so the results, are bit-identical to waiting for every group.
 // * epilogue: registers -> scale / bias -> global (optionally added into the output), and BatchNorm statistics:
 //   column sums over each warp's 16 rows by warp shuffles, the eight warps' sums combined in a fixed order, kept per
 //   CTA while the CTA stays on one channel block, one fp64 atomic pair per channel and flush.  No fp32 sum depends on
@@ -33,6 +34,7 @@
 #include "common.cuh"
 #include <cuda.h>
 #include <cstdlib>
+#include <type_traits>
 
 // ------------------------------------------------------------------------------------------
 // driver entry point for tensor-map encoding (no link-time dependency on libcuda)
@@ -369,13 +371,92 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         }
         st_s = 0.f; st_q = 0.f;
     };
+    // fp16 operands: the K loop of one tile.  It makes the adds of a loop that waits for every MMA group before it
+    // adds, on the same MMA chains and in the same order, so its results are bit-identical to that loop's; only the
+    // waits that order nothing are gone:
+    //   f16x3:  P1 part = hi*hi (k0,k1), C corr = lo*hi + hi*lo (k0..k3) | wait 1, acc += part        (C still runs)
+    //           P2 part = hi*hi (k2,k3)                                  | wait 0, acc += part + corr
+    //   f16:    P1 part = hi*hi (k0,k1) | wait 1, acc += corr (P2 of the previous stage)
+    //           P2 corr = hi*hi (k2,k3) | wait 1, acc += part
+    // The last add of an f16x3 stage needs its second hi*hi half and its corrections in registers at once, and at
+    // BN = 128 there is no room for a fourth register tile (acc, part, corr take 192 of the 232 registers), so that
+    // wait empties the queue; the other consumer warpgroup covers the gap.  In f16 a stage is read until its last
+    // group completes, which the first wait of the next stage (or the tile's final wait) proves: its `empty` arrive
+    // comes then.  The ring stays as it was: at BN = 128 three 64 KB stages fill the shared memory.
+    auto f16_tile = [&](auto split3_c) -> bool {
+        constexpr bool S3 = decltype(split3_c)::value;
+        uint32_t prev = 0;
+        for (int it = 0; it < iters; ++it) {
+            if (!__all_sync(0xffffffffu, mbar_wait(&full_bar[s], ph, err_flag, 2))) { wg_wait0(); return false; }
+            const uint32_t sa32 = smem_base + s * (uint32_t)stage_bytes;
+            const uint32_t arow = (uint32_t)cw * (TC_A_BYTES / 2);
+            const uint64_t da = sw128_desc(sa32 + arow), db = sw128_desc(sa32 + TC_A_BYTES);
+            const uint64_t dal = sw128_desc(sa32 + PER_OP + arow), dbl = sw128_desc(sa32 + PER_OP + TC_A_BYTES);
+            wg_arrive();
+            fence_regs(part);
+            if (S3) fence_regs(corr);
+#pragma unroll
+            for (int k = 0; k < 2; ++k) wgmma_op<BN, 1>(part, da + 2 * k, db + 2 * k, k);
+            wg_commit();
+            if (S3) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wgmma_op<BN, 1>(corr, dal + 2 * k, db + 2 * k, k);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wgmma_op<BN, 1>(corr, da + 2 * k, dbl + 2 * k, 1);
+                wg_commit();
+                asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+                fence_regs(part);
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+                wg_arrive();
+                fence_regs(part);
+#pragma unroll
+                for (int k = 2; k < 4; ++k) wgmma_op<BN, 1>(part, da + 2 * k, db + 2 * k, k - 2);
+                wg_commit();
+                wg_wait0();
+                fence_regs(part);
+                fence_regs(corr);
+                mbar_arrive(&empty_bar[s]);
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc[i] += part[i] + corr[i];
+            } else {
+                asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+                fence_regs(corr);
+                if (it > 0) {
+                    mbar_arrive(&empty_bar[prev]);
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) acc[i] += corr[i];
+                }
+                wg_arrive();
+                fence_regs(corr);
+#pragma unroll
+                for (int k = 2; k < 4; ++k) wgmma_op<BN, 1>(corr, da + 2 * k, db + 2 * k, k - 2);
+                wg_commit();
+                asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+                fence_regs(part);
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+            }
+            prev = s;
+            if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1u; }
+        }
+        if (!S3) {
+            wg_wait0();
+            fence_regs(corr);
+            mbar_arrive(&empty_bar[prev]);
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] += corr[i];
+        }
+        return true;
+    };
     for (int tile = blockIdx.x; tile < p.total_tiles && ok; tile += gridDim.x) {
         int n0, w0, h0, n;
         tc_tile_coords(p, tile, BN, n0, w0, h0, n);
         if (stats && n0 != st_n0) { flush_stats(); st_n0 = n0; }
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-        for (int it = 0; it < iters; ++it) {
+        if constexpr (F16 != 0) ok = split3 ? f16_tile(std::true_type{}) : f16_tile(std::false_type{});
+        else for (int it = 0; it < iters; ++it) {
             ok = __all_sync(0xffffffffu, mbar_wait(&full_bar[s], ph, err_flag, 2));
             if (!ok) break;
             uint8_t* sa = smem + (size_t)s * stage_bytes;
@@ -724,6 +805,8 @@ extern "C" int pxl_conv_tc_impl(const pxl_conv_geom* g, const int* taps, const f
 // A TMA box {one 128-byte row of channels, BW, BH, 1} of an NHWC tensor is (BW*BH pixel rows) x 128 B: both
 // operands arrive "MN-major" (the reduction index = pixel row is the slow one) in the SWIZZLE_128B layout.
 // * fp16 operands: wgmma reads MN-major fp16 directly (transpose bits set): 64-channel slabs, 16 pixel rows per MMA.
+//   The MMAs per stage (rows_alloc / 16: 1-4 in f16x3, 1-8 in f16) are a template constant of fully unrolled loop
+//   variants (a runtime trip count makes ptxas serialise the MMAs with extra warpgroup.arrive instructions).
 // * tf32 operands: wgmma takes tf32 K-major only, so the consumers transpose each stage (32 pixel rows) into a
 //   K-major tile in shared memory - splitting raw fp32 hi/lo for 3xTF32 in the same pass - and the MMAs read that.
 // Rows between BW*BH and the allocated rows are zeroed once and never written.  The pixel range is split over
@@ -831,71 +914,114 @@ conv_wgrad_wg_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_con
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     uint32_t s = 0, ph = 0;
     bool ok = true;
-    for (int it = 0; it < iters; ++it) {
+    if constexpr (F16 != 0) {
+        // fp16 operands: the K loop with KM = rows_alloc / 16 MMAs per operand pair and stage, fully unrolled.  A
+        // stage's hi*hi MMAs go into `part`, its f16x3 corrections into `corr`, and both are added once they are done.
+        auto f16_loop = [&](auto km_c, auto split3_c) -> bool {
+            constexpr int KM = decltype(km_c)::value;
+            constexpr bool S3 = decltype(split3_c)::value;
+            constexpr uint64_t kstep = (16 * 128) >> 4;            // 16 pixel rows per MMA
+            constexpr uint32_t SLAB = KM * 16 * 128;                // slab_bytes: rows_alloc = 16 KM
+            constexpr uint32_t PER_OP = (128 + BN) / 64 * SLAB;     // per_op: 64-channel slabs of dY and X
+            for (int it = 0; it < iters; ++it) {
+                if (!__all_sync(0xffffffffu, mbar_wait(&full_bar[s], ph, err_flag, 12))) return false;
+                const uint32_t sa32 = smem_base + s * (uint32_t)stage_bytes;
+                const uint32_t sb32 = sa32 + 2 * SLAB;
+                const uint64_t da = sw128_desc(sa32 + cw * SLAB, SLAB);
+                const uint64_t db = sw128_desc(sb32, SLAB);
+                wg_arrive();
+                fence_regs(part);
+                fence_regs(corr);
+#pragma unroll
+                for (int k = 0; k < KM; ++k) wgmma_op<BN, 2>(part, da + kstep * k, db + kstep * k, k);
+                if (S3) {
+                    const uint64_t dal = sw128_desc(sa32 + PER_OP + cw * SLAB, SLAB);
+                    const uint64_t dbl = sw128_desc(sb32 + PER_OP, SLAB);
+#pragma unroll
+                    for (int k = 0; k < KM; ++k) wgmma_op<BN, 2>(corr, dal + kstep * k, db + kstep * k, k);
+#pragma unroll
+                    for (int k = 0; k < KM; ++k) wgmma_op<BN, 2>(corr, da + kstep * k, dbl + kstep * k, 1);
+                }
+                wg_commit();
+                wg_wait0();
+                fence_regs(part);
+                fence_regs(corr);
+                mbar_arrive(&empty_bar[s]);
+                if (S3) {
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) acc[i] += part[i] + corr[i];
+                } else {
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+                }
+                if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1u; }
+            }
+            return true;
+        };
+        // rows_alloc <= 64 for f16x3 and <= 128 for f16 (conv_wgrad_tc_core's maxrows)
+        using std::integral_constant;
+        using T = std::true_type;
+        using F = std::false_type;
+        if (split3) {
+            switch (p.rows_alloc / 16) {
+                case 1: ok = f16_loop(integral_constant<int, 1>{}, T{}); break;
+                case 2: ok = f16_loop(integral_constant<int, 2>{}, T{}); break;
+                case 3: ok = f16_loop(integral_constant<int, 3>{}, T{}); break;
+                default: ok = f16_loop(integral_constant<int, 4>{}, T{}); break;
+            }
+        } else {
+            switch (p.rows_alloc / 16) {
+                case 1: ok = f16_loop(integral_constant<int, 1>{}, F{}); break;
+                case 2: ok = f16_loop(integral_constant<int, 2>{}, F{}); break;
+                case 3: ok = f16_loop(integral_constant<int, 3>{}, F{}); break;
+                case 4: ok = f16_loop(integral_constant<int, 4>{}, F{}); break;
+                case 5: ok = f16_loop(integral_constant<int, 5>{}, F{}); break;
+                case 6: ok = f16_loop(integral_constant<int, 6>{}, F{}); break;
+                case 7: ok = f16_loop(integral_constant<int, 7>{}, F{}); break;
+                default: ok = f16_loop(integral_constant<int, 8>{}, F{}); break;
+            }
+        }
+    } else for (int it = 0; it < iters; ++it) {
         ok = __all_sync(0xffffffffu, mbar_wait(&full_bar[s], ph, err_flag, 12));
         if (!ok) break;
         uint8_t* sa = smem + (size_t)s * stage_bytes;
-        const uint32_t sa32 = smem_base + s * (uint32_t)stage_bytes;
-        if constexpr (F16 != 0) {
-            const int kmma = p.rows_alloc / 16;
-            const uint32_t sb32 = sa32 + (uint32_t)(slabsA * slab_bytes);
-            const uint64_t da = sw128_desc(sa32 + (uint32_t)(cw * slab_bytes), (uint32_t)slab_bytes);
-            const uint64_t db = sw128_desc(sb32, (uint32_t)slab_bytes);
-            const uint64_t dal = sw128_desc(sa32 + (uint32_t)per_op + (uint32_t)(cw * slab_bytes), (uint32_t)slab_bytes);
-            const uint64_t dbl = sw128_desc(sb32 + (uint32_t)per_op, (uint32_t)slab_bytes);
-            const uint64_t kstep = (16 * 128) >> 4;            // 16 pixel rows per MMA
-            wg_arrive();
-            fence_regs(part);
-            fence_regs(corr);
-            for (int k = 0; k < kmma; ++k) wgmma_op<BN, 2>(part, da + kstep * k, db + kstep * k, k);
-            if (split3) {
-                for (int k = 0; k < kmma; ++k) wgmma_op<BN, 2>(corr, dal + kstep * k, db + kstep * k, k);
-                for (int k = 0; k < kmma; ++k) wgmma_op<BN, 2>(corr, da + kstep * k, dbl + kstep * k, 1);
-            }
-            wg_commit();
-            wg_wait0();
-            fence_regs(part);
-            fence_regs(corr);
-            mbar_arrive(&empty_bar[s]);
-        } else {
-            // transpose the stage (32 pixel rows) into K-major tiles: unit u = (channel row R, pixels 4g .. 4g+3)
-            named_bar(1, 256);                                // both warpgroups are done reading the previous tiles
-            const int units = (128 + BN) * 8;
-            for (int u = ct; u < units; u += 256) {
-                const int R = u >> 3, g = u & 7;
-                const int slab = R < 128 ? (R >> 5) : slabsA + ((R - 128) >> 5);
-                const int c = R & 31;
-                const uint8_t* src = sa + (size_t)slab * slab_bytes + (c & 3) * 4;
-                float4 v, vl = make_float4(0.f, 0.f, 0.f, 0.f);
-                float* vp = &v.x; float* lp = &vl.x;
+        // transpose the stage (32 pixel rows) into K-major tiles: unit u = (channel row R, pixels 4g .. 4g+3)
+        named_bar(1, 256);                                // both warpgroups are done reading the previous tiles
+        const int units = (128 + BN) * 8;
+        for (int u = ct; u < units; u += 256) {
+            const int R = u >> 3, g = u & 7;
+            const int slab = R < 128 ? (R >> 5) : slabsA + ((R - 128) >> 5);
+            const int c = R & 31;
+            const uint8_t* src = sa + (size_t)slab * slab_bytes + (c & 3) * 4;
+            float4 v, vl = make_float4(0.f, 0.f, 0.f, 0.f);
+            float* vp = &v.x; float* lp = &vl.x;
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const int px = 4 * g + e;
-                    const int off = px * 128 + ((((c >> 2) ^ (px & 7))) << 4);
-                    vp[e] = *reinterpret_cast<const float*>(src + off);
-                    if (split3 && !p.inkernel) lp[e] = *reinterpret_cast<const float*>(src + per_op + off);
-                }
-                if (p.inkernel) v = tf32_split4(v, vl);
-                const int doff = R * 128 + ((g ^ (R & 7)) << 4);
-                *reinterpret_cast<float4*>(kt + doff) = v;
-                if (split3) *reinterpret_cast<float4*>(kt + KT_BYTES + doff) = vl;
+            for (int e = 0; e < 4; ++e) {
+                const int px = 4 * g + e;
+                const int off = px * 128 + ((((c >> 2) ^ (px & 7))) << 4);
+                vp[e] = *reinterpret_cast<const float*>(src + off);
+                if (split3 && !p.inkernel) lp[e] = *reinterpret_cast<const float*>(src + per_op + off);
             }
-            fence_async_smem();
-            named_bar(1, 256);
-            mbar_arrive(&empty_bar[s]);                      // the ring slot has been copied out
-            const uint32_t k32 = smem_u32(kt);
-            const uint32_t arow = (uint32_t)cw * 64 * 128;
-            const uint64_t da = sw128_desc(k32 + arow), db = sw128_desc(k32 + 128 * 128);
-            const uint64_t dal = sw128_desc(k32 + KT_BYTES + arow), dbl = sw128_desc(k32 + KT_BYTES + 128 * 128);
-            wg_arrive();
-            fence_regs(part);
-            fence_regs(corr);
-            mma_slice<BN, 0>(part, corr, da, db, dal, dbl, split3);
-            wg_commit();
-            wg_wait0();
-            fence_regs(part);
-            fence_regs(corr);
+            if (p.inkernel) v = tf32_split4(v, vl);
+            const int doff = R * 128 + ((g ^ (R & 7)) << 4);
+            *reinterpret_cast<float4*>(kt + doff) = v;
+            if (split3) *reinterpret_cast<float4*>(kt + KT_BYTES + doff) = vl;
         }
+        fence_async_smem();
+        named_bar(1, 256);
+        mbar_arrive(&empty_bar[s]);                      // the ring slot has been copied out
+        const uint32_t k32 = smem_u32(kt);
+        const uint32_t arow = (uint32_t)cw * 64 * 128;
+        const uint64_t da = sw128_desc(k32 + arow), db = sw128_desc(k32 + 128 * 128);
+        const uint64_t dal = sw128_desc(k32 + KT_BYTES + arow), dbl = sw128_desc(k32 + KT_BYTES + 128 * 128);
+        wg_arrive();
+        fence_regs(part);
+        fence_regs(corr);
+        mma_slice<BN, 0>(part, corr, da, db, dal, dbl, split3);
+        wg_commit();
+        wg_wait0();
+        fence_regs(part);
+        fence_regs(corr);
         if (split3) {
 #pragma unroll
             for (int i = 0; i < BN / 2; ++i) acc[i] += part[i] + corr[i];
