@@ -76,6 +76,22 @@ int pxl_cps_ce(const float* s_l, const float* s_r, const float* t_l, const float
                float* grad_l, float* grad_r, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * UniMatch (Yang et al., CVPR 2023) thresholded pseudo-label loss.  Planar [*, C, H, W] maps, C <= 32:
+ *   w    [ubs]       weak-view logits (pseudo-label = first maximal index, confidence = its softmax)
+ *   mix  [ubs]       pseudo-label source inside the boxes: row i uses mix[(i - mix_shift) mod ubs]
+ *   s    [2*ubs]     strong-view logits, view k of image i at row k*ubs + i
+ *   fp   [lbs+ubs]   feature-perturbed logits; rows lbs.. are the unlabeled images
+ *   boxes            DEVICE int32 [2*ubs][4] = y0, x0, y1, x1 per strong view (16-byte aligned; empty: y0 == y1)
+ * L_v = sum over pixels with confidence >= tau of CE(pred_v, label) / (ubs*H*W), v in {s1, s2, fp};
+ * out[4] = L_s1, L_s2, L_fp, number of weak-view pixels with confidence >= tau.
+ * grad_s [2*ubs] and grad_fp [lbs+ubs] receive w_v * dL_v/dpred (zero for the labeled fp rows).
+ * Sums in a fixed order: repeated calls are bit-identical.
+ * ------------------------------------------------------------------------------------------- */
+int pxl_unimatch_ce(const float* w, const float* mix, const float* s, const float* fp, const int* boxes,
+                    int ubs, int lbs, int mix_shift, int C, int H, int W, float tau, float w_s1,
+                    float w_s2, float w_fp, float* out, float* grad_s, float* grad_fp, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Channel softmax on planar maps: F.softmax(pred, dim=1), task/sseg/model.py:62,121;
  * task/sseg/func.py:216-220
  * ------------------------------------------------------------------------------------------- */
@@ -355,6 +371,10 @@ int pxl_pixel_shuffle2_nhwc(const float* in, float* out, int N, int h, int w, in
  * chan_scale[n,c] * (1 + elem_noise[hw,c]), every factor nullable */
 int pxl_perturb_nhwc(const float* x, const float* pixel_mask, const float* chan_scale, const float* elem_noise,
                      float* out, int N, int64_t HW, int C, void* stream);
+/* UniMatch feature perturbation on an NHWC map: out [2N,HW,C] = [x; x * chan_scale[n,c]]; backward
+ * dx = grad[:N] + grad[N:] * chan_scale.  C % 4 == 0. */
+int pxl_fp_dup_nhwc(const float* x, const float* chan_scale, float* out, int N, int64_t HW, int C, void* stream);
+int pxl_fp_dup_bwd_nhwc(const float* grad, const float* chan_scale, float* dx, int N, int64_t HW, int C, void* stream);
 int pxl_channel_mean_nhwc(const float* x, float* out, int64_t pixels, int C, void* stream);
 int pxl_argmax_nonzero_mask(const float* logits, float* mask, int n, int C, int64_t HW, void* stream);
 
@@ -449,6 +469,15 @@ int pxl_input_prehandle(const uint8_t* img_hwc, const uint8_t* lab_hw, int H, in
                         const int* lx, const int* ly, int x1, int y1, int crop_w, int crop_h, int flip,
                         float label_fill, float label_const, const double* mean3_host, const double* std3_host,
                         float* out_img_chw, float* out_lab_hw, void* stream);
+
+/* ---- UniMatch strong augmentation (csrc/strong_aug.cu) ------------------------------------------------------
+ * weak [ubs,3,H,W] normalised planar images -> out [2*ubs,3,H,W]: view k of image i at row k*ubs + i.  Per view
+ * (DEVICE float table [2*ubs][32], drawn by the host): de-normalise and clamp to [0,1], ColorJitter in the drawn
+ * order, grayscale, Gaussian blur (reflect padding), paste of the partner image's same view (image (i + ubs/2) mod
+ * ubs) inside the box, renormalise - torchvision's float-tensor semantics.  tmp_a / tmp_b: [2*ubs,3,H,W] scratch;
+ * gray_mean [2*ubs]: the contrast means.  H, W > 6. */
+int pxl_strong_aug(const float* weak, const float* table, int ubs, int H, int W, const double* mean3_host,
+                   const double* std3_host, float* out, float* tmp_a, float* tmp_b, float* gray_mean, void* stream);
 
 #ifdef __cplusplus
 }

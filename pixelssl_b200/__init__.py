@@ -10,23 +10,30 @@ from .version import __version__
 from .utils import log_info, log_warn, log_err, str2bool, str2intlist, REGRESSION, CLASSIFICATION
 from . import nn, ssl_algorithm
 from .ssl_algorithm import (SSL_NULL, SSL_MT, SSL_ADV, SSL_S4L, SSL_GCT, SSL_CCT, SSL_CUTMIX, SSL_CPS,
-                            SSL_ALGORITHMS)
+                            SSL_UNIMATCH, SSL_ALGORITHMS, EXTRA_SSL_ALGORITHMS, ALL_SSL_ALGORITHMS)
 from .runner import create_parser, build_args, run_script
 
 
-def register_into_pixelssl(pixelssl_module=None, task_sseg_modules=None):
+def register_into_pixelssl(pixelssl_module=None, task_sseg_modules=None, extra_algorithms=()):
     """Drop the engine in under an unmodified ``pixelssl.runner`` / ``TaskProxy``: replaces the
     algorithm modules TaskProxy looks up by name (task_template/proxy.py:433-434), adds the ones
     PixelSSL does not have (``ssl_cps``) to ``pixelssl.ssl_algorithm.SSL_ALGORITHMS`` (the list
     ``pixelssl.runner.create_parser`` checks names against) and, if the task's ``model`` /
-    ``criterion`` modules are given, replaces their export functions (proxy.py:426-427)."""
+    ``criterion`` modules are given, replaces their export functions (proxy.py:426-427).
+
+    ``extra_algorithms``: names from ``EXTRA_SSL_ALGORITHMS`` (``ssl_unimatch``) to install and list as well.  They
+    are opt-in so that the algorithm list an existing integration sees stays the one it had."""
+    unknown = [n for n in extra_algorithms if n not in EXTRA_SSL_ALGORITHMS]
+    if unknown:
+        raise ValueError('register_into_pixelssl: unknown extra algorithms {0}; available: {1}'.format(
+            unknown, EXTRA_SSL_ALGORITHMS))
     if pixelssl_module is None:
         import pixelssl as pixelssl_module
     names = getattr(pixelssl_module.ssl_algorithm, 'SSL_ALGORITHMS', None)
     if names is None:
         names = []
         pixelssl_module.ssl_algorithm.SSL_ALGORITHMS = names
-    for name in SSL_ALGORITHMS:
+    for name in SSL_ALGORITHMS + [n for n in EXTRA_SSL_ALGORITHMS if n in extra_algorithms]:
         mod = getattr(ssl_algorithm, name)
         pixelssl_module.ssl_algorithm.__dict__[name] = mod
         setattr(pixelssl_module.ssl_algorithm, name, mod)

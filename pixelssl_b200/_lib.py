@@ -37,6 +37,8 @@ SIGNATURES = {
     'pxl_mse_consistency_bwd': (c_int, [P, P, c_int64, c_float, P, P, P]),
     'pxl_ce2d': (c_int, [P, P, c_int, c_int, c_int64, c_int, P, P, P, c_float, P]),
     'pxl_cps_ce': (c_int, [P, P, P, P, c_int, c_int, c_int64, c_float, P, P, P, P]),
+    'pxl_unimatch_ce': (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float, c_float,
+                                P, P, P, P]),
     'pxl_softmax_planar': (c_int, [P, P, c_int, c_int, c_int64, P]),
     'pxl_softmax_planar_bwd': (c_int, [P, P, P, c_int, c_int, c_int64, P]),
     'pxl_softmax_mse': (c_int, [P, P, c_int, c_int, c_int64, c_float, P, P, P, P, P]),
@@ -95,6 +97,8 @@ SIGNATURES = {
     'pxl_fdgt_absdiff': (c_int, [P, P, c_float, c_int, c_int, c_int64, P, P]),
     'pxl_pixel_shuffle2_nhwc': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     'pxl_perturb_nhwc': (c_int, [P, P, P, P, P, c_int, c_int64, c_int, P]),
+    'pxl_fp_dup_nhwc': (c_int, [P, P, P, c_int, c_int64, c_int, P]),
+    'pxl_fp_dup_bwd_nhwc': (c_int, [P, P, P, c_int, c_int64, c_int, P]),
     'pxl_channel_mean_nhwc': (c_int, [P, P, c_int64, c_int, P]),
     'pxl_argmax_nonzero_mask': (c_int, [P, P, c_int, c_int, c_int64, P]),
     'pxl_adaptive_avgpool_nhwc': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P]),
@@ -122,6 +126,7 @@ SIGNATURES = {
     'pxl_s4l_rotate_batch': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, P]),
     'pxl_input_prehandle': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, P, c_int, P, P, c_int, c_int, c_int, c_int,
                                     c_int, c_float, c_float, P, P, P, P, P]),
+    'pxl_strong_aug': (c_int, [P, P, c_int, c_int, c_int, P, P, P, P, P, P, P]),
     'pxl_sgd_ema': (c_int, [P, P, P, P, c_int64, c_float, c_float, c_float, c_float, c_int, P]),
     'pxl_ema': (c_int, [P, P, c_int64, c_float, P]),
 }

@@ -489,6 +489,57 @@ extern "C" int pxl_perturb_nhwc(const float* x, const float* pixel_mask, const f
     return 0;
 }
 
+// UniMatch feature perturbation: out [2N, HW, C] = [x; x * chan_scale[n, c]] (Dropout2d copies after the clean
+// features, one read and two writes); backward dx = g[:N] + g[N:] * chan_scale.  Products and sums are rounded
+// separately, as torch's x * s and a + b * s are.
+__global__ void __launch_bounds__(256)
+fp_dup_kernel(const float4* __restrict__ x, const float* __restrict__ cscale, float4* __restrict__ out, int64_t n4,
+              int c4, int64_t HW) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+        const int c = (int)(i % c4);
+        const int64_t n = i / c4 / HW;
+        const float4 s = __ldg(reinterpret_cast<const float4*>(cscale) + n * c4 + c);
+        const float4 v = x[i];
+        out[i] = v;
+        out[n4 + i] = make_float4(__fmul_rn(v.x, s.x), __fmul_rn(v.y, s.y), __fmul_rn(v.z, s.z), __fmul_rn(v.w, s.w));
+    }
+}
+
+__global__ void __launch_bounds__(256)
+fp_dup_bwd_kernel(const float4* __restrict__ g, const float* __restrict__ cscale, float4* __restrict__ dx, int64_t n4,
+                  int c4, int64_t HW) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+        const int c = (int)(i % c4);
+        const int64_t n = i / c4 / HW;
+        const float4 s = __ldg(reinterpret_cast<const float4*>(cscale) + n * c4 + c);
+        const float4 a = g[i], b = g[n4 + i];
+        dx[i] = make_float4(__fadd_rn(a.x, __fmul_rn(b.x, s.x)), __fadd_rn(a.y, __fmul_rn(b.y, s.y)),
+                            __fadd_rn(a.z, __fmul_rn(b.z, s.z)), __fadd_rn(a.w, __fmul_rn(b.w, s.w)));
+    }
+}
+
+extern "C" int pxl_fp_dup_nhwc(const float* x, const float* chan_scale, float* out, int N, int64_t HW, int C,
+                               void* stream) {
+    if (!x || !chan_scale || !out || N <= 0 || HW <= 0 || C <= 0 || (C & 3)) return PXL_ERR_BAD_ARG;
+    const int64_t n4 = (int64_t)N * HW * (C / 4);
+    fp_dup_kernel<<<ew_blocks(n4), 256, 0, (cudaStream_t)stream>>>((const float4*)x, chan_scale, (float4*)out, n4,
+                                                                   C / 4, HW);
+    PXL_CHECK_LAUNCH();
+    return 0;
+}
+
+extern "C" int pxl_fp_dup_bwd_nhwc(const float* grad, const float* chan_scale, float* dx, int N, int64_t HW, int C,
+                                   void* stream) {
+    if (!grad || !chan_scale || !dx || N <= 0 || HW <= 0 || C <= 0 || (C & 3)) return PXL_ERR_BAD_ARG;
+    const int64_t n4 = (int64_t)N * HW * (C / 4);
+    fp_dup_bwd_kernel<<<ew_blocks(n4), 256, 0, (cudaStream_t)stream>>>((const float4*)grad, chan_scale, (float4*)dx,
+                                                                       n4, C / 4, HW);
+    PXL_CHECK_LAUNCH();
+    return 0;
+}
+
 // mean over channels per pixel of an NHWC tensor: FeatureDropDecoder attention (ssl_cct.py:721)
 __global__ void __launch_bounds__(256)
 channel_mean_kernel(const float* __restrict__ x, float* __restrict__ out, int64_t pixels, int C) {

@@ -410,6 +410,139 @@ extern "C" int pxl_cps_ce(const float* s_l, const float* s_r, const float* t_l, 
 }
 
 // ------------------------------------------------------------------------------------------
+// UniMatch thresholded pseudo-label loss (Yang et al., CVPR 2023).  One thread per pixel of each
+// unlabeled image i.  The weak view's logits w[i] give the pixel's pseudo-label (first maximal
+// index) and confidence (its largest softmax probability).  Strong view k (rows k*ubs + i of s)
+// takes label and confidence from w_mix[i] = mix[(i - mix_shift) mod ubs] inside its box and from
+// w[i] elsewhere; the FP map (row lbs + i of fp) always from w[i].  Each term is
+//   L_v = sum over confident pixels of CE(pred_v, label) / (ubs * HW)
+// and its gradient, scaled by the term's weight, is written in the same pass (zero where the
+// pixel is not confident).  Blocks with blockIdx.y >= ubs zero the gradient of the labeled FP rows.
+//   algorithmic traffic: read w, s1, s2, fp + w_mix inside the boxes, write three gradients:
+//   about 32*C B/pixel; strong / FP logits of unconfident pixels are not read.
+// fp64 per-block partials of (L_s1, L_s2, L_fp, confident count), summed in a fixed order by
+// unimatch_sum_kernel: no atomics, repeated calls are bit-identical.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ void unimatch_label(const float* __restrict__ t, int C, int64_t HW, int& y, float& conf) {
+    float v[CE_MAXC];
+    float m = 0.f;
+    y = 0;
+#pragma unroll
+    for (int c = 0; c < CE_MAXC; ++c)
+        if (c < C) {
+            v[c] = t[(int64_t)c * HW];
+            if (c == 0 || cps_beats(v[c], m)) { m = v[c]; y = c; }
+        }
+    float se = 0.f;
+#pragma unroll
+    for (int c = 0; c < CE_MAXC; ++c)
+        if (c < C) se += expf(v[c] - m);
+    conf = 1.f / se;                        // softmax of the maximal channel: exp(0) / sum
+}
+
+// masked cross-entropy of one pixel: loss (0 if not confident) and its gradient (zero if not confident)
+__device__ __forceinline__ float unimatch_term(const float* __restrict__ x, float* __restrict__ gp, int C, int64_t HW,
+                                               int y, bool confident, float g) {
+    if (!confident) {
+#pragma unroll
+        for (int c = 0; c < CE_MAXC; ++c)
+            if (c < C) gp[(int64_t)c * HW] = 0.f;
+        return 0.f;
+    }
+    float v[CE_MAXC];
+#pragma unroll
+    for (int c = 0; c < CE_MAXC; ++c)
+        if (c < C) v[c] = x[(int64_t)c * HW];
+    return cps_pixel<true>(v, C, y, g, gp, HW);
+}
+
+__global__ void __launch_bounds__(256)
+unimatch_ce_kernel(const float* __restrict__ w, const float* __restrict__ mix, const float* __restrict__ s,
+                   const float* __restrict__ fp, const int* __restrict__ boxes, int ubs, int lbs, int mix_shift, int C,
+                   int W, int64_t HW, float tau, float g_s1, float g_s2, float g_fp, double* __restrict__ part,
+                   float* __restrict__ grad_s, float* __restrict__ grad_fp) {
+    const int i = blockIdx.y;
+    const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= ubs) {                           // labeled FP rows take no part in the loss: zero gradient
+        if (p < HW) {
+            float* gp = grad_fp + (int64_t)(i - ubs) * C * HW + p;
+            for (int c = 0; c < C; ++c) gp[(int64_t)c * HW] = 0.f;
+        }
+        return;                               // block-uniform
+    }
+    double acc[4] = {0.0, 0.0, 0.0, 0.0};
+    if (p < HW) {
+        const int py = (int)(p / W), px = (int)(p - (int64_t)py * W);
+        const int64_t plane = (int64_t)C * HW;
+        int yw;
+        float cw;
+        unimatch_label(w + i * plane + p, C, HW, yw, cw);
+        acc[3] = cw >= tau ? 1.0 : 0.0;
+        const int r = ((i - mix_shift) % ubs + ubs) % ubs;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const int v = k * ubs + i;
+            const int4 b = __ldg(reinterpret_cast<const int4*>(boxes) + v);     // y0, x0, y1, x1
+            int y = yw;
+            float conf = cw;
+            if (py >= b.x && py < b.z && px >= b.y && px < b.w) unimatch_label(mix + r * plane + p, C, HW, y, conf);
+            acc[k] = (double)unimatch_term(s + v * plane + p, grad_s + v * plane + p, C, HW, y, conf >= tau,
+                                           k == 0 ? g_s1 : g_s2);
+        }
+        const int64_t f = (int64_t)(lbs + i) * plane + p;
+        acc[2] = (double)unimatch_term(fp + f, grad_fp + f, C, HW, yw, cw >= tau, g_fp);
+    }
+    __shared__ double wp[4][8];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const double v = warp_sum_d(acc[q]);
+        if ((threadIdx.x & 31) == 0) wp[q][threadIdx.x >> 5] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < 4) {
+        double t = 0.0;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) t += wp[threadIdx.x][k];
+        part[((int64_t)threadIdx.x * ubs + i) * gridDim.x + blockIdx.x] = t;
+    }
+}
+
+// out[q] = (sum of term q's ubs * nblk partials) * (q < 3 ? inv_n : 1).  Warp q: lane j adds partials j, j+32, ...
+// in order, then a fixed shuffle tree.  The count is an integer below 2^24, exact in fp32.
+__global__ void __launch_bounds__(128)
+unimatch_sum_kernel(const double* __restrict__ part, int64_t per_term, double inv_n, float* __restrict__ out) {
+    const int q = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double s = 0.0;
+    for (int64_t k = lane; k < per_term; k += 32) s += __ldg(part + q * per_term + k);
+    s = warp_sum_d(s);
+    if (lane == 0) out[q] = (float)(q < 3 ? s * inv_n : s);
+}
+
+extern "C" int pxl_unimatch_ce(const float* w, const float* mix, const float* s, const float* fp, const int* boxes,
+                               int ubs, int lbs, int mix_shift, int C, int H, int W, float tau, float w_s1,
+                               float w_s2, float w_fp, float* out, float* grad_s, float* grad_fp, void* stream) {
+    if (!w || !mix || !s || !fp || !boxes || !out || !grad_s || !grad_fp) return PXL_ERR_BAD_ARG;
+    if (ubs <= 0 || lbs < 0 || C <= 0 || H <= 0 || W <= 0) return PXL_ERR_BAD_ARG;
+    if (C > CE_MAXC || ubs + lbs > 65535) return PXL_ERR_UNSUPPORTED;
+    if ((reinterpret_cast<uintptr_t>(boxes) & 15) != 0) return PXL_ERR_BAD_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t HW = (int64_t)H * W;
+    dim3 grid((unsigned)pxl_cdiv(HW, 256), (unsigned)(ubs + lbs));
+    const int64_t per_term = (int64_t)ubs * grid.x;
+    int rc = 0;
+    double* part = (double*)pxl_workspace_(PXL_WS_UNIMATCH, stream, (size_t)(4 * per_term) * sizeof(double), &rc);
+    if (rc) return rc;
+    const double n = (double)ubs * (double)HW;
+    unimatch_ce_kernel<<<grid, 256, 0, st>>>(w, mix, s, fp, boxes, ubs, lbs, mix_shift, C, W, HW, tau,
+                                             (float)((double)w_s1 / n), (float)((double)w_s2 / n),
+                                             (float)((double)w_fp / n), part, grad_s, grad_fp);
+    PXL_CHECK_LAUNCH();
+    unimatch_sum_kernel<<<1, 128, 0, st>>>(part, per_term, 1.0 / n, out);
+    PXL_CHECK_LAUNCH();
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------
 // channel softmax fwd / bwd on planar maps (task/sseg/model.py:62)
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)

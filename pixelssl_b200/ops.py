@@ -271,6 +271,104 @@ def cps_cross_entropy(s_l, s_r, t_l=None, t_r=None, loss_scale=1.0, unit_upstrea
     return _CpsCrossEntropy.apply(s_l, s_r, t_l, t_r, float(loss_scale), bool(unit_upstream))
 
 
+def unimatch_raw(w, mix, s, pred_fp, fp_offset, boxes, threshold, weights, mix_shift):
+    """One pxl_unimatch_ce launch.  Returns (out[4] = L_s1, L_s2, L_fp, confident count; grad_s; grad_fp), the
+    gradients scaled by ``weights``.  The timer metadata of the launch is its algorithmic traffic in bytes: w, s1, s2
+    and the unlabeled FP rows read, w_mix read inside the boxes, three gradients written and the labeled FP rows
+    zeroed."""
+    ubs, c, h, wd = w.shape
+    out = torch.empty(4, dtype=torch.float32, device=w.device)
+    grad_s = torch.empty_like(s)
+    grad_fp = torch.empty_like(pred_fp)
+    b = boxes.cpu() if boxes.is_cuda else boxes
+    mix_px = int(((b[:, 2] - b[:, 0]).clamp_min(0) * (b[:, 3] - b[:, 1]).clamp_min(0)).sum())
+    meta = 4 * c * (7 * ubs * h * wd + mix_px + fp_offset * h * wd)
+    boxes = boxes.to(dtype=torch.int32).contiguous().to(device=w.device, non_blocking=True)
+    _timed_call('pxl_unimatch_ce', _p(w), _p(mix), _p(s), _p(pred_fp), _p(boxes), ubs, int(fp_offset), int(mix_shift),
+                c, h, wd, float(threshold), float(weights[0]), float(weights[1]), float(weights[2]), _p(out),
+                _p(grad_s), _p(grad_fp), _stream(), meta=meta)
+    return out, grad_s, grad_fp
+
+
+class _UnimatchCrossEntropy(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, s, pred_fp, w, mix, boxes, fp_offset, threshold, weights, mix_shift, unit_upstream):
+        ws = weights if unit_upstream else (1.0, 1.0, 1.0)
+        out, grad_s, grad_fp = unimatch_raw(w, mix, s, pred_fp, fp_offset, boxes, threshold, ws, mix_shift)
+        ctx.unit = unit_upstream
+        ctx.save_for_backward(grad_s, grad_fp)
+        return out[0], out[1], out[2], out[3]
+
+    @staticmethod
+    def backward(ctx, g1, g2, gf, _):
+        grad_s, grad_fp = ctx.saved_tensors
+        if not ctx.unit:
+            g1, g2, gf = (0.0 if g is None else g for g in (g1, g2, gf))
+            ubs = grad_s.shape[0] // 2
+            grad_s = torch.cat([grad_s[:ubs] * g1, grad_s[ubs:] * g2])
+            grad_fp = grad_fp * gf
+        return grad_s, grad_fp, None, None, None, None, None, None, None, None
+
+
+def unimatch_cross_entropy(s, pred_fp, w, mix, boxes, threshold, weights=(1.0, 1.0, 1.0), fp_offset=None,
+                           mix_shift=None, unit_upstream=False):
+    """UniMatch's thresholded pseudo-label cross-entropy (Yang et al., CVPR 2023) -> (L_s1, L_s2, L_fp, count), four
+    0-d tensors.
+
+    w: the weak view's logits [ubs,C,H,W]; each pixel's pseudo-label is its first maximal index and its confidence
+    the largest softmax probability.  s: the strong views' logits [2*ubs,C,H,W] (view 1 rows, then view 2 rows).
+    pred_fp: the feature-perturbed logits of the whole batch [fp_offset+ubs,C,H,W] (default fp_offset: the labeled
+    rows in front of the ubs unlabeled ones).  Inside view k's box ``boxes[k*ubs + i]`` (y0, x0, y1, x1; an int
+    tensor [2*ubs,4], empty when y0 == y1) the label and confidence of s come from ``torch.roll(mix, mix_shift, 0)``
+    (default shift ubs/2).  L_v = sum of CE over pixels with confidence >= threshold / (ubs*H*W); count is the number
+    of weak-view pixels with confidence >= threshold.  w and mix are never differentiated.
+    unit_upstream=True: the caller guarantees d total / d L_v == weights[v], so the forward launch writes the
+    gradients (about 32*C B/pixel).  Otherwise backward scales unit-weight gradients by the upstream gradients.
+    Inputs must be fp32, CUDA, contiguous planar maps with C <= 32."""
+    w, mix = w.detach(), mix.detach()
+    for t, name in ((s, 's'), (pred_fp, 'pred_fp'), (w, 'w'), (mix, 'mix')):
+        _chk(t, name)
+        if t.dim() != 4:
+            raise ValueError('%s: expected a planar [n,C,H,W] map, got shape %s' % (name, tuple(t.shape)))
+    ubs = w.shape[0]
+    if fp_offset is None:
+        fp_offset = pred_fp.shape[0] - ubs
+    per = tuple(w.shape[1:])
+    if mix.shape != w.shape or s.shape != (2 * ubs,) + per or pred_fp.shape != (fp_offset + ubs,) + per:
+        raise ValueError('unimatch_cross_entropy: shapes w %s mix %s s %s pred_fp %s (fp_offset %d) do not fit' % (
+            tuple(w.shape), tuple(mix.shape), tuple(s.shape), tuple(pred_fp.shape), fp_offset))
+    if tuple(boxes.shape) != (2 * ubs, 4):
+        raise ValueError('boxes: expected shape (%d, 4), got %s' % (2 * ubs, tuple(boxes.shape)))
+    if len(weights) != 3:
+        raise ValueError('weights: expected three loss weights (s1, s2, fp)')
+    mix_shift = ubs // 2 if mix_shift is None else int(mix_shift)
+    return _UnimatchCrossEntropy.apply(s, pred_fp, w, mix, boxes, int(fp_offset), float(threshold),
+                                       tuple(float(x) for x in weights), mix_shift, bool(unit_upstream))
+
+
+def strong_aug(weak, table):
+    """UniMatch's strong augmentation of a batch of normalised planar images on the device.
+    weak [ubs,3,H,W] (normalised with the input pipeline's MEAN / STD); table [2*ubs,32] float32 per-view parameters
+    (ssl_algorithm/ssl_unimatch.py draws them; layout in csrc/strong_aug.cu) -> (views [2*ubs,3,H,W]: view 1 of every
+    image, then view 2; gray_mean [2*ubs]: the grayscale means contrast blended with).  Five launches for the batch;
+    the timer metadata is the bytes they move: per view the source image read twice, two scratch maps written and
+    read, the view written."""
+    from .task.sseg.gpu_input import _MEAN_C, _STD_C
+    _chk(weak, 'weak')
+    ubs, c, h, w = weak.shape
+    if c != 3:
+        raise ValueError('strong_aug expects 3-channel images, got %d channels' % c)
+    table = table.to(device=weak.device, dtype=torch.float32).contiguous()
+    if tuple(table.shape) != (2 * ubs, 32):
+        raise ValueError('table: expected shape (%d, 32), got %s' % (2 * ubs, tuple(table.shape)))
+    out = torch.empty((2 * ubs, 3, h, w), dtype=torch.float32, device=weak.device)
+    tmp_a, tmp_b = torch.empty_like(out), torch.empty_like(out)
+    gray_mean = torch.empty(2 * ubs, dtype=torch.float32, device=weak.device)
+    _timed_call('pxl_strong_aug', _p(weak), _p(table), ubs, h, w, _MEAN_C, _STD_C, _p(out), _p(tmp_a), _p(tmp_b),
+                _p(gray_mean), _stream(), meta=4 * 3 * h * w * 2 * ubs * 7)
+    return out, gray_mean
+
+
 class _Softmax(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits):
@@ -1792,6 +1890,40 @@ def perturb(x, pixel_mask=None, chan_scale=None, elem_noise=None):
     if elem_noise is not None:
         elem_noise = elem_noise.permute(1, 2, 0).contiguous()
     return _Perturb.apply(as_cl(x), pixel_mask, chan_scale, elem_noise)
+
+
+class _FpDup(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, chan_scale):
+        n, c, h, w = x.shape
+        out = torch.empty((2 * n, c, h, w), dtype=x.dtype, device=x.device, memory_format=CL)
+        call('pxl_fp_dup_nhwc', _p(x), _p(chan_scale), _p(out), n, h * w, c, _stream())
+        ctx.save_for_backward(chan_scale)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        (chan_scale,) = ctx.saved_tensors
+        g = as_cl(g)
+        n, c, h, w = g.shape
+        dx = torch.empty((n // 2, c, h, w), dtype=g.dtype, device=g.device, memory_format=CL)
+        call('pxl_fp_dup_bwd_nhwc', _p(g), _p(chan_scale), _p(dx), n // 2, h * w, c, _stream())
+        return dx, None
+
+
+def fp_dup(x, chan_scale):
+    """UniMatch's feature perturbation: ``torch.cat([x, x * chan_scale[:, :, None, None]])`` of a channels_last
+    [n,C,H,W] map in one launch -> channels_last [2n,C,H,W]; the backward, ``g[:n] + g[n:] * chan_scale``, is one
+    launch too.  chan_scale [n,C] holds the Dropout2d factors (0 or 1/(1-p)); it is not differentiated."""
+    x = as_cl(x)
+    _chk(x, 'x', cl=True)
+    chan_scale = chan_scale.detach().contiguous()
+    _chk(chan_scale, 'chan_scale')
+    if chan_scale.shape != x.shape[:2]:
+        raise ValueError('chan_scale: expected shape %s, got %s' % (tuple(x.shape[:2]), tuple(chan_scale.shape)))
+    if x.shape[1] % 4:
+        raise ValueError('fp_dup needs a channel count divisible by 4, got %d' % x.shape[1])
+    return _FpDup.apply(x, chan_scale)
 
 
 def channel_mean(x):

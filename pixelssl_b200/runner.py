@@ -13,9 +13,9 @@ from .utils import cmd, logger
 
 def create_parser(algorithm):
     parser = argparse.ArgumentParser(description='PixelSSL-H100 Static Script Parser')
-    if algorithm not in ssl_algorithm.SSL_ALGORITHMS:
+    if algorithm not in ssl_algorithm.ALL_SSL_ALGORITHMS:
         logger.log_err('Unknown semi-supervised learning algorithm: {0}\n'
-                       'The support algorithms are: {1}\n'.format(algorithm, ssl_algorithm.SSL_ALGORITHMS))
+                       'The support algorithms are: {1}\n'.format(algorithm, ssl_algorithm.ALL_SSL_ALGORITHMS))
     optimizer.add_parser_arguments(parser)
     lrer.add_parser_arguments(parser)
     getattr(ssl_algorithm, algorithm).add_parser_arguments(parser)

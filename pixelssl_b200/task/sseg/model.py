@@ -109,6 +109,24 @@ class DeepLabV2(TaskModel):
         resulter['sslcct_ad_inp'] = latent
         return resulter, debugger
 
+    @property
+    def fp_channels(self):
+        """Channel counts of the feature maps ``forward_fp`` perturbs, in the order of its ``scales``."""
+        return self.model.FP_CHANNELS
+
+    def forward_fp(self, inp, scales):
+        """UniMatch's forward with feature perturbation: ``scales`` holds one [n, C] tensor of Dropout2d factors per
+        entry of ``fp_channels``.  -> (resulter of the clean features, resulter of the perturbed ones); the head
+        runs once on both, so its BatchNorm statistics cover both."""
+        if not len(inp) == 1:
+            logger.log_err('Semantic segmentation model DeepLab requires only one input\n'
+                           'However, {0} inputs are given\n'.format(len(inp)))
+        pred, pred_fp, latent = self.model.forward_fp(inp[0], scales)
+        resulter = {'pred': (pred,), 'activated_pred': LazyActivation(pred), 'ssls4l_rc_inp': pred,
+                    'sslcct_ad_inp': latent}
+        resulter_fp = {'pred': (pred_fp,), 'activated_pred': LazyActivation(pred_fp)}
+        return resulter, resulter_fp
+
 
 class DeepLabV3Plus(DeepLabV2):
     """DeepLabV3+ with the DeepLabV2 plugin surface: same backbones, resulter keys and latent (the layer4 output);

@@ -41,6 +41,20 @@ class DeepLabV2(nn.Module):
         x = ops.bilinear(low, img.shape[2:], align_corners=True, channels=self.num_classes, nhwc=True)
         return x, bx
 
+    # the feature maps forward_fp perturbs, in the order of its ``scales``: the layer4 output the classifier reads
+    FP_CHANNELS = (2048,)
+
+    def forward_fp(self, img, scales):
+        """UniMatch's feature-perturbation forward: the classifier runs once on ``[bx; bx * scales[0]]`` (Dropout2d
+        factors [n, 2048]) -> (pred, pred_fp, latent).  Each half is upsampled on its own, so the backward
+        never splits a full-resolution map."""
+        n = img.shape[0]
+        bx = self.backbone(img)
+        low = self.classifier(ops.fp_dup(bx, scales[0]))
+        up = [ops.bilinear(low[k * n:(k + 1) * n], img.shape[2:], align_corners=True, channels=self.num_classes,
+                           nhwc=True) for k in (0, 1)]
+        return up[0], up[1], bx
+
     # No train() override: like the reference (deeplab_v2.py:46-52, model.py:69-80) freeze_bn() is applied once at
     # construction and is undone by the .train() call that starts every epoch; BN layers that ARE in eval mode inside
     # a training graph are supported by ops.bn_act (running statistics as constants in the backward).

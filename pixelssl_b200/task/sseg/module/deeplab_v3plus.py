@@ -151,6 +151,22 @@ class DeepLabV3Plus(nn.Module):
         x = ops.bilinear(x, img.shape[2:], align_corners=True, channels=self.num_classes, nhwc=True)
         return x, bx
 
+    # the feature maps forward_fp perturbs, in the order of its ``scales``: layer1 (the decoder's low-level input) and
+    # layer4 (the ASPP input), as UniMatch drops both
+    FP_CHANNELS = (256, 2048)
+
+    def forward_fp(self, img, scales):
+        """UniMatch's feature-perturbation forward: the head runs once on the clean features followed by their
+        Dropout2d copies (``scales``: factors [n, 256] for layer1 and [n, 2048] for layer4) -> (pred, pred_fp,
+        latent).  Each half is upsampled on its own, so the backward never splits a full-resolution map."""
+        n = img.shape[0]
+        low, bx = self.backbone.forward_low_level(img)
+        x = self.decoder(self.aspp(ops.fp_dup(bx, scales[1])), ops.fp_dup(low, scales[0]))
+        x = self.classifier(x)
+        up = [ops.bilinear(x[k * n:(k + 1) * n], img.shape[2:], align_corners=True, channels=self.num_classes,
+                           nhwc=True) for k in (0, 1)]
+        return up[0], up[1], bx
+
     # No train() override, as in DeepLabV2: freeze_bn() applies once at construction.
 
     def freeze_bn(self):
