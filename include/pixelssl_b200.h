@@ -92,6 +92,32 @@ int pxl_unimatch_ce(const float* w, const float* mix, const float* s, const floa
                     float w_s2, float w_fp, float* out, float* grad_s, float* grad_fp, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * OHEM cross-entropy: the probability OHEM of ProbOhemCrossEntropy2d (the supervised term of CPS and
+ * UniMatch).  logits planar [n, C, HW] (C <= 32), labels fp32 [n, HW]; a pixel is valid as in
+ * pxl_ce2d.  q = softmax(logits)[y] on valid pixels and 1 on the others; V = number of valid pixels.
+ * k = min_kept: if k == 0, k > V or V == 0 every valid pixel is kept; else t_k = k-th smallest q
+ * over all n*HW pixels (NaN last), T = t_k if t_k > thresh else thresh, and a pixel is kept when it
+ * is valid and q <= T.  K = number of kept pixels.
+ *   per_sample[i] = n * sum over kept pixels of image i of (logsumexp - x_y) / K   (NaN if K == 0)
+ *   grad_logits (nullable) = g * n / K * (softmax - onehot) on kept pixels, 0 elsewhere, with
+ *   g = upstream_const (pxl_ohem_ce) or upstream[i] (pxl_ohem_ce_bwd).
+ * q (out, [n, HW]) receives the q map; stats (out, fp64 [4]) = V, K, T, t_k (T = +inf when every
+ * valid pixel is kept; t_k NaN when the selection was not needed).  Both stay on the device and
+ * nothing is copied to the host; the call synchronises only when its scratch buffer grows (the
+ * first call, or a batch with more pixels than any earlier one on the stream: cudaFree +
+ * cudaMalloc, as for pxl_ce2d / pxl_cps_ce).  pxl_ohem_ce_bwd recomputes the loss and writes the
+ * gradient from the q map and stats of a pxl_ohem_ce call.  thresh must be finite, min_kept >= 0,
+ * n*HW < 2^32 (else PXL_ERR_UNSUPPORTED).
+ * Sums are taken in a fixed order: repeated calls are bit-identical.
+ * ------------------------------------------------------------------------------------------- */
+int pxl_ohem_ce(const float* logits, const float* labels, int n, int C, int64_t HW, int ignore_index,
+                float thresh, int64_t min_kept, float* per_sample, float* grad_logits,
+                float upstream_const, float* q, double* stats, void* stream);
+int pxl_ohem_ce_bwd(const float* logits, const float* labels, const float* q, const double* stats,
+                    int n, int C, int64_t HW, int ignore_index, const float* upstream,
+                    float* per_sample, float* grad_logits, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Channel softmax on planar maps: F.softmax(pred, dim=1), task/sseg/model.py:62,121;
  * task/sseg/func.py:216-220
  * ------------------------------------------------------------------------------------------- */

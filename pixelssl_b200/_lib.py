@@ -39,6 +39,8 @@ SIGNATURES = {
     'pxl_cps_ce': (c_int, [P, P, P, P, c_int, c_int, c_int64, c_float, P, P, P, P]),
     'pxl_unimatch_ce': (c_int, [P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float, c_float,
                                 P, P, P, P]),
+    'pxl_ohem_ce': (c_int, [P, P, c_int, c_int, c_int64, c_int, c_float, c_int64, P, P, c_float, P, P, P]),
+    'pxl_ohem_ce_bwd': (c_int, [P, P, P, P, c_int, c_int, c_int64, c_int, P, P, P, P]),
     'pxl_softmax_planar': (c_int, [P, P, c_int, c_int, c_int64, P]),
     'pxl_softmax_planar_bwd': (c_int, [P, P, P, c_int, c_int, c_int64, P]),
     'pxl_softmax_mse': (c_int, [P, P, c_int, c_int, c_int64, c_float, P, P, P, P, P]),

@@ -9,6 +9,7 @@ Conventions
 All tensors must be fp32 CUDA tensors; anything else raises (no silent fallback)."""
 import ctypes
 import functools
+import math
 
 import torch
 
@@ -210,6 +211,84 @@ def cross_entropy2d(logits, gt, ignore_index=255, upstream_const=None):
     (e.g. 1/n when ``torch.mean`` of the result goes straight into the loss) and the gradient is
     written by the forward launch."""
     return _CrossEntropy2d.apply(logits.contiguous(), gt.contiguous(), ignore_index, upstream_const)
+
+
+def ohem_bytes(n, c, hw, kept, selected, with_grad):
+    """Algorithmic traffic in bytes of one pxl_ohem_ce call with ``kept`` (K) kept pixels: the pixel pass reads the
+    logits and labels and writes q (4C + 8 B/pixel); when the radix selection runs (``selected``: t_k is not NaN in
+    the stats) its two refinement passes read q (4 B/pixel each); the loss pass reads q and the labels (8 B/pixel) and
+    the logits of the kept pixels only (4C B each), and writes the gradient of every pixel (4C B/pixel) if asked."""
+    N = n * hw
+    return N * (4 * c + 8) + (8 * N if selected else 0) + 8 * N + 4 * c * kept + (4 * c * N if with_grad else 0)
+
+
+def ohem_raw(logits, gt, ignore_index, thresh, min_kept, upstream_const=None):
+    """One pxl_ohem_ce call.  Returns (per_sample[n], grad or None, q map [n,H,W], stats [4] fp64 = V, K, T, t_k), all
+    on the device.  The gradient is written when ``upstream_const`` is given.  The timer metadata of the call is the
+    part of its algorithmic traffic the host knows without waiting for the device: ``ohem_bytes`` with no kept pixel
+    and no selection.  ``ohem_bytes`` with K and t_k from ``stats`` gives the whole traffic."""
+    _chk(logits, 'logits')
+    if logits.dim() != 4:
+        raise ValueError('logits: expected a planar [n,C,H,W] map, got shape %s' % (tuple(logits.shape),))
+    n, c, h, w = logits.shape
+    gt = _labels_flat(gt, n, h * w)
+    thresh, min_kept = float(thresh), int(min_kept)
+    if not math.isfinite(thresh) or min_kept < 0:
+        raise ValueError('ohem: thresh must be finite and min_kept >= 0 (got %r, %r)' % (thresh, min_kept))
+    per = torch.empty(n, dtype=torch.float32, device=logits.device)
+    grad = torch.empty_like(logits) if upstream_const is not None else None
+    q = torch.empty((n, h, w), dtype=torch.float32, device=logits.device)
+    stats = torch.empty(4, dtype=torch.float64, device=logits.device)
+    meta = ohem_bytes(n, c, h * w, 0, False, grad is not None)
+    _timed_call('pxl_ohem_ce', _p(logits), _p(gt), n, c, h * w, int(ignore_index), thresh, min_kept, _p(per), _p(grad),
+                float(upstream_const or 0.0), _p(q), _p(stats), _stream(), meta=meta)
+    return per, grad, q, stats
+
+
+class _OhemCrossEntropy2d(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, gt, ignore_index, thresh, min_kept, upstream_const):
+        need = ctx.needs_input_grad[0]
+        fused = need and upstream_const is not None
+        per, grad, q, stats = ohem_raw(logits, gt, ignore_index, thresh, min_kept, upstream_const if fused else None)
+        ctx.fused, ctx.ignore = fused, int(ignore_index)
+        if need:
+            if fused:
+                ctx.save_for_backward(grad)
+            else:
+                ctx.save_for_backward(logits, gt, q, stats)
+        return per
+
+    @staticmethod
+    def backward(ctx, g):
+        if ctx.fused:
+            (grad,) = ctx.saved_tensors
+            return grad, None, None, None, None, None
+        logits, gt, q, stats = ctx.saved_tensors
+        n, c, h, w = logits.shape
+        per = torch.empty(n, dtype=torch.float32, device=logits.device)
+        grad = torch.empty_like(logits)
+        g = g.contiguous().float()
+        # timer metadata: q, labels and the gradient; the logits of the kept pixels (4C B each) come on top
+        _timed_call('pxl_ohem_ce_bwd', _p(logits), _p(gt), _p(q), _p(stats), n, c, h * w, ctx.ignore, _p(g), _p(per),
+                    _p(grad), _stream(), meta=n * h * w * (4 * c + 8))
+        return grad, None, None, None, None, None
+
+
+def ohem_cross_entropy2d(logits, gt, ignore_index, thresh, min_kept, upstream_const=None):
+    """Probability-OHEM cross-entropy (ProbOhemCrossEntropy2d, as CPS and UniMatch train their supervised term) ->
+    per-sample loss [n] whose ``torch.mean`` is the OHEM loss.
+
+    q = softmax(logits)[y] on valid pixels (as ``cross_entropy2d``'s), 1 on the others.  With k = min_kept and V valid
+    pixels in the batch: if k == 0 or k > V every valid pixel is kept; else t_k is the k-th smallest q over every pixel
+    of the batch, T = max(t_k, thresh) (thresh when t_k is NaN) and the valid pixels with q <= T are kept.  The loss is
+    the mean CE over the K kept pixels (NaN when V == 0); per_sample[i] = n * (CE summed over image i's kept pixels) / K.
+    The selection stays on the device and nothing is copied to the host; as for ``cross_entropy2d``, only the growth
+    of the kernels' scratch buffer (a first call, or more pixels than any earlier call) synchronises the device.
+    upstream_const: as ``cross_entropy2d``'s (1/n when ``torch.mean`` of the result goes straight into the loss), the
+    gradient is then written by the forward call."""
+    return _OhemCrossEntropy2d.apply(logits.contiguous(), gt.contiguous(), ignore_index, thresh, min_kept,
+                                     upstream_const)
 
 
 def cps_raw(s_l, s_r, t_l, t_r, grad_scale, want_grad):

@@ -72,6 +72,12 @@ def build_args(config, iters_per_epoch=100):
     """config dict (as in task/sseg/script/*.py) -> argparse.Namespace with the autoset fields."""
     parser = create_parser(config['ssl_algorithm'])
     add_proxy_arguments(parser)
+    crits = config.get('criterions') or {}
+    if isinstance(crits, str):
+        crits = yaml.full_load(crits) or {}
+    from .task.sseg import criterion as sseg_criterion
+    if any(v in sseg_criterion.OHEM_CRITERIONS for v in crits.values()):
+        sseg_criterion.add_ohem_parser_arguments(parser)
     if 'pretrained_backbone' not in config:
         config = dict(config, pretrained_backbone='none')     # programmatic builds (tests, bench): synthetic weights
     args = cmd.parse_args(parser, config)
