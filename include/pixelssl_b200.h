@@ -505,6 +505,27 @@ int pxl_input_prehandle(const uint8_t* img_hwc, const uint8_t* lab_hw, int H, in
 int pxl_strong_aug(const float* weak, const float* table, int ubs, int H, int W, const double* mean3_host,
                    const double* std3_host, float* out, float* tmp_a, float* tmp_b, float* gray_mean, void* stream);
 
+/* ---- multi-view evaluation (csrc/eval_views.cu; task/sseg/evaluation.py) ----------------------------------------
+ * A view of x [n,3,H,W] is x resized to hv x wv (bilinear, align_corners=True; a copy when hv x wv == H x W), flipped
+ * along W if flip.  Its tiles start at rows k*sh (k*sh < hv) and columns l*sw (l*sw < wv) and are clipped to the
+ * view; 'whole' is the single tile gh = sh = hv, gw = sw = wv.  Tiles of one shape form a group; groups are numbered
+ * (row class, column class) row-class major, where the classes of an axis are [full-length tiles (if any), then each
+ * clipped tail in order] - at most three per axis, at most nine groups.  A group's tiles are the row-major product of
+ * its nr rows (r0 + i*sh) and nc columns (c0 + j*sw); tile t of sample b is row t*n + b of its tensors.
+ * pxl_eval_tiles: out [nr*nc*n, 3, th, tw] = one group's tiles, read straight from x.
+ * pxl_eval_merge: group_logits_host[ngroups] = DEVICE pointers of the groups' logits [T*n, C, th, tw]; out [n,C,hv,wv]
+ * (accumulate: +=) = per view pixel the sum of softmax over the tiles covering it, in row-major tile order, written
+ * un-flipped.  C <= 32.
+ * pxl_eval_view_add: S [n,C,H,W] (accumulate: +=) = bilinear_ac(P [n,C,hv,wv]).  C <= 32.
+ * pxl_eval_finish: mean = S / V, logmean = log(max(mean, FLT_MIN)) over count values. */
+int pxl_eval_tiles(const float* x, float* out, int n, int H, int W, int hv, int wv, int flip, int r0, int nr, int c0,
+                   int nc, int sh, int sw, int th, int tw, void* stream);
+int pxl_eval_merge(const float* const* group_logits_host, int ngroups, int n, int C, int hv, int wv, int gh, int gw,
+                   int sh, int sw, int flip, int accumulate, float* out, void* stream);
+int pxl_eval_view_add(const float* P, float* S, int n, int C, int hv, int wv, int H, int W, int accumulate,
+                      void* stream);
+int pxl_eval_finish(const float* S, float* mean, float* logmean, int64_t count, int V, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

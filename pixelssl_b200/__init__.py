@@ -14,7 +14,8 @@ from .ssl_algorithm import (SSL_NULL, SSL_MT, SSL_ADV, SSL_S4L, SSL_GCT, SSL_CCT
 from .runner import create_parser, build_args, run_script
 
 
-def register_into_pixelssl(pixelssl_module=None, task_sseg_modules=None, extra_algorithms=(), extra_criterions=()):
+def register_into_pixelssl(pixelssl_module=None, task_sseg_modules=None, extra_algorithms=(), extra_criterions=(),
+                           val_protocol=False):
     """Drop the engine in under an unmodified ``pixelssl.runner`` / ``TaskProxy``: replaces the
     algorithm modules TaskProxy looks up by name (task_template/proxy.py:433-434), adds the ones
     PixelSSL does not have (``ssl_cps``) to ``pixelssl.ssl_algorithm.SSL_ALGORITHMS`` (the list
@@ -26,7 +27,11 @@ def register_into_pixelssl(pixelssl_module=None, task_sseg_modules=None, extra_a
 
     ``extra_criterions``: names from ``task.sseg.criterion.OHEM_CRITERIONS`` (``ohem_sseg_criterion``) to install into
     the task's criterion module (``task_sseg_modules[1]``), whose ``add_parser_arguments`` then also adds their flags
-    (``--ohem-thresh``, ``--ohem-min-kept``).  Opt-in for the same reason: the default parser stays PixelSSL's."""
+    (``--ohem-thresh``, ``--ohem-min-kept``).  Opt-in for the same reason: the default parser stays PixelSSL's.
+
+    ``val_protocol``: the task's model module's (``task_sseg_modules[0]``) ``add_parser_arguments`` also adds the
+    multi-view validation flags (``--val-protocol``, ``--val-crop-size``, ``--val-scales``, ``--val-flip``;
+    task/sseg/evaluation.py).  Opt-in for the same reason."""
     from .task.sseg import criterion as b200_criterion
     unknown = [n for n in extra_algorithms if n not in EXTRA_SSL_ALGORITHMS]
     if unknown:
@@ -38,6 +43,9 @@ def register_into_pixelssl(pixelssl_module=None, task_sseg_modules=None, extra_a
             unknown, b200_criterion.OHEM_CRITERIONS))
     if extra_criterions and task_sseg_modules is None:
         raise ValueError('register_into_pixelssl: extra_criterions are installed into the task\'s criterion module; '
+                         'pass task_sseg_modules')
+    if val_protocol and task_sseg_modules is None:
+        raise ValueError('register_into_pixelssl: the val_protocol flags are added by the task\'s model module; '
                          'pass task_sseg_modules')
     if pixelssl_module is None:
         import pixelssl as pixelssl_module
@@ -72,6 +80,16 @@ def register_into_pixelssl(pixelssl_module=None, task_sseg_modules=None, extra_a
                 b200_criterion.add_ohem_parser_arguments(parser)
             add_parser_arguments.adds_ohem_flags = True
             task_criterion.add_parser_arguments = add_parser_arguments
+        model_base = getattr(task_model, 'add_parser_arguments', None)
+        if val_protocol and not getattr(model_base, 'adds_val_protocol_flags', False):
+            from .task.sseg import evaluation as b200_evaluation
+
+            def add_model_parser_arguments(parser):
+                if model_base is not None:
+                    model_base(parser)
+                b200_evaluation.add_val_protocol_parser_arguments(parser)
+            add_model_parser_arguments.adds_val_protocol_flags = True
+            task_model.add_parser_arguments = add_model_parser_arguments
         if len(task_sseg_modules) > 2:
             # optional third module = the task's func.py: validation metrics on the GPU (confusion matrix kernel);
             # the reference's own TaskFunc keeps working too (it moves the probability map to the host)

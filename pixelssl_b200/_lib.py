@@ -131,6 +131,12 @@ SIGNATURES = {
     'pxl_strong_aug': (c_int, [P, P, c_int, c_int, c_int, P, P, P, P, P, P, P]),
     'pxl_sgd_ema': (c_int, [P, P, P, P, c_int64, c_float, c_float, c_float, c_float, c_int, P]),
     'pxl_ema': (c_int, [P, P, c_int64, c_float, P]),
+    'pxl_eval_tiles': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                               c_int, P]),
+    'pxl_eval_merge': (c_int, [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                               c_int, P, P]),
+    'pxl_eval_view_add': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
+    'pxl_eval_finish': (c_int, [P, P, P, c_int64, c_int, P]),
 }
 
 PXL_ERR_BAD_ARG = -1

@@ -3,18 +3,7 @@
 // Output (and grad_out) are planar [n, C, H, W]; the small input is planar or NHWC (ldc stride).
 // Forward is write-bound: 4*C B per output pixel.  The source-index arithmetic mirrors ATen's
 // area_pixel_compute_source_index so results agree to fp32 round-off.
-#include "common.cuh"
-
-__device__ __forceinline__ float src_index(float scale, int dst, bool align_corners) {
-    if (align_corners) return scale * (float)dst;
-    float s = scale * ((float)dst + 0.5f) - 0.5f;
-    return s < 0.f ? 0.f : s;
-}
-
-static inline float resize_scale(int in, int out, int align_corners) {
-    if (align_corners) return out > 1 ? (float)(in - 1) / (float)(out - 1) : 0.f;
-    return (float)in / (float)out;
-}
+#include "resample.cuh"
 
 #define BL_MAXC 32
 template <bool NHWC>

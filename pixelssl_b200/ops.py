@@ -2169,6 +2169,73 @@ def confusion_matrix_(cmat, pred, gt, num_classes=None):
     return cmat
 
 
+# ------------------------------------------------------------------------------------------------
+# multi-view evaluation (csrc/eval_views.cu, task/sseg/evaluation.py)
+# ------------------------------------------------------------------------------------------------
+# The timer metadata of each launch is its algorithmic traffic: every value written once, every value read once
+# (the neighbours a bilinear tap shares with an adjacent output are not counted again).
+
+def eval_tiles(x, hv, wv, flip, r0, nr, c0, nc, sh, sw, th, tw):
+    """One shape group of a view's tiles: x [n,3,H,W] resized to hv x wv (bilinear, align_corners=True; a copy at the
+    same size), flipped along W if ``flip``, tiles at rows r0 + i*sh (i < nr) and columns c0 + j*sw (j < nc), th x tw
+    each -> [nr*nc*n, 3, th, tw], tile t of sample b at row t*n + b."""
+    _chk(x, 'x')
+    n, c, H, W = x.shape
+    if c != 3:
+        raise ValueError('eval_tiles expects 3-channel images, got %d channels' % c)
+    T = int(nr) * int(nc)
+    out = torch.empty((T * n, 3, int(th), int(tw)), dtype=torch.float32, device=x.device)
+    _timed_call('pxl_eval_tiles', _p(x), _p(out), n, H, W, int(hv), int(wv), int(bool(flip)), int(r0), int(nr), int(c0),
+                int(nc), int(sh), int(sw), int(th), int(tw), _stream(), meta=2 * 4 * out.numel())
+    return out
+
+
+def eval_merge(group_logits, n, hv, wv, gh, gw, sh, sw, flip, out=None, accumulate=False):
+    """Sum over the covering tiles of softmax(tile logits) per view pixel, in row-major tile order, un-flipped if
+    ``flip``.  group_logits: one planar [T*n, C, th, tw] tensor per shape group in the order of
+    ``evaluation.tile_groups``.  -> out [n,C,hv,wv] (written, or added to if ``accumulate``; a new tensor if None)."""
+    if not group_logits:
+        raise ValueError('eval_merge needs the logits of at least one tile group')
+    for i, g in enumerate(group_logits):
+        _chk(g, 'group_logits[%d]' % i)
+    C = group_logits[0].shape[1]
+    if any(g.dim() != 4 or g.shape[1] != C for g in group_logits):
+        raise ValueError('every group\'s logits must be [T*n, %d, th, tw]' % C)
+    if out is None:
+        out = torch.empty((n, C, int(hv), int(wv)), dtype=torch.float32, device=group_logits[0].device)
+        accumulate = False
+    else:
+        _chk(out, 'out')
+        if tuple(out.shape) != (n, C, int(hv), int(wv)):
+            raise ValueError('out must be [%d, %d, %d, %d], got %s' % (n, C, hv, wv, tuple(out.shape)))
+    ptrs = (ctypes.c_void_p * len(group_logits))(*[g.data_ptr() for g in group_logits])
+    moved = 4 * (sum(g.numel() for g in group_logits) + (2 if accumulate else 1) * out.numel())
+    _timed_call('pxl_eval_merge', ptrs, len(group_logits), int(n), int(C), int(hv), int(wv), int(gh), int(gw), int(sh),
+                int(sw), int(bool(flip)), int(bool(accumulate)), _p(out), _stream(), meta=moved)
+    return out
+
+
+def eval_view_add(P, S, accumulate=True):
+    """S [n,C,H,W] += (or = unless ``accumulate``) the bilinear (align_corners=True) resize of P [n,C,hv,wv]."""
+    _chk(P, 'P')
+    _chk(S, 'S')
+    n, C, hv, wv = P.shape
+    if S.dim() != 4 or S.shape[0] != n or S.shape[1] != C:
+        raise ValueError('S must be [%d, %d, H, W], got %s' % (n, C, tuple(S.shape)))
+    H, W = S.shape[2:]
+    moved = 4 * (P.numel() + (2 if accumulate else 1) * S.numel())
+    _timed_call('pxl_eval_view_add', _p(P), _p(S), n, C, hv, wv, H, W, int(bool(accumulate)), _stream(), meta=moved)
+    return S
+
+
+def eval_finish(S, V):
+    """-> (S / V, log(max(S / V, FLT_MIN))) in one launch."""
+    _chk(S, 'S')
+    mean, logmean = torch.empty_like(S), torch.empty_like(S)
+    _timed_call('pxl_eval_finish', _p(S), _p(mean), _p(logmean), S.numel(), int(V), _stream(), meta=12 * S.numel())
+    return mean, logmean
+
+
 _GN_WS = {}
 
 

@@ -78,6 +78,9 @@ def build_args(config, iters_per_epoch=100):
     from .task.sseg import criterion as sseg_criterion
     if any(v in sseg_criterion.OHEM_CRITERIONS for v in crits.values()):
         sseg_criterion.add_ohem_parser_arguments(parser)
+    from .task.sseg import evaluation as sseg_evaluation
+    if any(k in config for k in sseg_evaluation.FLAGS):
+        sseg_evaluation.add_val_protocol_parser_arguments(parser)
     if 'pretrained_backbone' not in config:
         config = dict(config, pretrained_backbone='none')     # programmatic builds (tests, bench): synthetic weights
     args = cmd.parse_args(parser, config)

@@ -4,6 +4,7 @@
 ``SUPPORTED_TASK_TYPES``.  TaskProxy (task_template/proxy.py:134-159,433-441) only ever touches
 these."""
 from ..utils import logger
+from ..task.sseg import evaluation
 
 
 def add_parser_arguments(parser):
@@ -21,6 +22,7 @@ class _SSLBase:
         self.models, self.optimizers, self.lrers, self.criterions = {}, {}, {}, {}
 
     def build(self, model_funcs, optimizer_funcs, lrer_funcs, criterion_funcs, task_func):
+        evaluation.check_args(self.args)
         self._build(model_funcs, optimizer_funcs, lrer_funcs, criterion_funcs, task_func)
 
     def train(self, data_loader, epoch):
@@ -28,8 +30,12 @@ class _SSLBase:
         self._flush_log()
 
     def validate(self, data_loader, epoch):
+        """``_validate`` inside the multi-view evaluation scope: an eval-mode task model then forwards the views of
+        ``--val-protocol`` / ``--val-scales`` / ``--val-flip`` (task/sseg/evaluation.py); the default protocol changes
+        nothing."""
         self._flush_log()
-        self._validate(data_loader, epoch)
+        with evaluation.validating():
+            self._validate(data_loader, epoch)
 
     def _log_step(self, make_line):
         """The per-step log line of every reference ``_train`` (e.g. ssl_mt.py:199-207), emitted ONE logging

@@ -1,11 +1,13 @@
 """Task-model plugin for semantic segmentation: the contract of task/sseg/model.py:11-125
 (export fns ``deeplabv2()`` / ``pspnet()``, plus ``deeplabv3plus()``, ``cls(args)``, ``.param_groups``,
 ``forward(inp: tuple) -> (resulter, debugger)`` with 'pred', 'activated_pred', 'ssls4l_rc_inp',
-'sslcct_ad_inp')."""
+'sslcct_ad_inp').  Inside validation with a multi-view protocol, ``forward`` of an eval-mode model returns the
+ensemble of task/sseg/evaluation.py instead (no 'sslcct_ad_inp')."""
 import torch.nn as nn
 
 from ... import ops
 from ...utils import logger, cmd
+from . import evaluation
 from .module import deeplab_v2, deeplab_v3plus, pspnet as pspnet_module
 
 
@@ -102,6 +104,8 @@ class DeepLabV2(TaskModel):
         if not len(inp) == 1:
             logger.log_err('Semantic segmentation model DeepLab requires only one input\n'
                            'However, {0} inputs are given\n'.format(len(inp)))
+        if evaluation.multi_view(self):
+            return evaluation.forward_views(self, inp)
         pred, latent = self.model(inp[0])
         resulter['pred'] = (pred,)
         resulter['activated_pred'] = LazyActivation(pred)
@@ -155,6 +159,8 @@ class PSPNet(TaskModel):
         if not len(inp) == 1:
             logger.log_err('Semantic segmentation model PSPNet requires only one input\n'
                            'However, {0} inputs are given\n'.format(len(inp)))
+        if evaluation.multi_view(self):
+            return evaluation.forward_views(self, inp)
         pred, latent = self.model(inp[0])
         resulter['pred'] = (pred,)
         resulter['activated_pred'] = LazyActivation(pred)
