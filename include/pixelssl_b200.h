@@ -336,6 +336,9 @@ int pxl_stem_conv7x7s2_wgrad(const float* img_planar, const float* dy, float* dw
 /* im2col of the stem for the tensor-core path: cols [N*OH*OW][160], k = (r*7+s)*3+c (the weight's physical
  * order), lanes 147..159 zero; the stem then is a flat 1x1 convolution with 160 input lanes */
 int pxl_stem_im2col(const float* img_planar, float* cols, int N, int H, int W, int OH, int OW, void* stream);
+/* im2col of the deep stem's first convolution (3x3 stride 2 pad 1, 3 -> 64): cols [N*OH*OW][32],
+ * k = (r*3+s)*3+c, lanes 27..31 zero */
+int pxl_stem3x3s2_im2col(const float* img_planar, float* cols, int N, int H, int W, int OH, int OW, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Optimiser + EMA on flat parameter arenas:
@@ -450,6 +453,9 @@ int pxl_peer_status(void);
 /* stem im2col written directly as the fp16 pair [pixels][192] of the f16 wgmma path (hi, lo nullable; value*scale) */
 int pxl_stem_im2col_h16(const float* img_planar, void* hi, void* lo, float scale, int N, int H, int W, int OH, int OW,
                         void* stream);
+/* the same for the deep stem's 3x3/2 pad 1 convolution: fp16 pair [pixels][64], lanes 27..63 zero */
+int pxl_stem3x3s2_im2col_h16(const float* img_planar, void* hi, void* lo, float scale, int N, int H, int W, int OH,
+                             int OW, void* stream);
 
 /* ---- ASPP head as one GEMM + gather (csrc/aspp_gather.cu) ----------------------------------------------------
  * Classifier_Module.forward (task/sseg/module/deeplab_v2.py:81-85) = sum of four dilated 3x3 convolutions 2048 -> C.

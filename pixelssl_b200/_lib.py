@@ -85,6 +85,7 @@ SIGNATURES = {
     'pxl_stem_conv7x7s2': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, P]),
     'pxl_stem_conv7x7s2_wgrad': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, P]),
     'pxl_stem_im2col': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P]),
+    'pxl_stem3x3s2_im2col': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P]),
     'pxl_planar_to_nhwc': (c_int, [P, P, c_int, c_int, c_int64, c_int, c_int, P]),
     'pxl_nhwc_to_planar': (c_int, [P, P, c_int, c_int, c_int64, c_int, c_int, P]),
     'pxl_onehot_nhwc': (c_int, [P, P, c_int64, c_int, c_int, c_int, P]),
@@ -119,6 +120,7 @@ SIGNATURES = {
                                       c_int, P, P, P, P, P, P, P]),
     'pxl_peer_status': (c_int, []),
     'pxl_stem_im2col_h16': (c_int, [P, P, P, c_float, c_int, c_int, c_int, c_int, c_int, P]),
+    'pxl_stem3x3s2_im2col_h16': (c_int, [P, P, P, c_float, c_int, c_int, c_int, c_int, c_int, P]),
     'pxl_aspp_gather': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int), c_int, P]),
     'pxl_aspp_scatter_h16': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int), c_int, P]),
     'pxl_lane_concat_nhwc': (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_int), c_int, P, c_int, c_int, c_int, c_int, P]),

@@ -609,26 +609,32 @@ extern "C" int pxl_stem_conv7x7s2_wgrad(const float* img, const float* dy, float
 }
 
 // ------------------------------------------------------------------------------------------
-// stem im2col for the tensor-core path: cols[pixel][k], k = (r*7 + s)*3 + c for k < 147 (the physical
-// order of the channels_last [64,3,7,7] weight), zero for 147 <= k < 160.  The 7x7/2 stem then runs as a
-// flat 1x1 convolution with 160 input lanes on wgmma (forward and wgrad share the matrix).
+// stem im2col for the tensor-core path: cols[pixel][k], k = (r*KS + s)*3 + c for k < 3*KS*KS (the physical order of
+// the channels_last [64,3,KS,KS] weight), zero up to the lane count KP.  The stride-2 stem then runs as a flat 1x1
+// convolution with KP input lanes on wgmma (forward and wgrad share the matrix).  Geometries: the 7x7/2 pad 3 stem
+// (147 + 13 zero lanes = 160) and the deep stem's first 3x3/2 pad 1 convolution (27 + 5 zero lanes = 32, the tf32
+// kernels' channel multiple).
 // ------------------------------------------------------------------------------------------
 #define ST_KP 160
+#define ST3_K 27
+#define ST3_KP 32
+template <int KS, int PAD, int KP>
 __global__ void __launch_bounds__(256)
 stem_im2col_kernel(const float* __restrict__ img, float* __restrict__ cols, int N, int H, int W, int OH, int OW) {
-    const int64_t total4 = (int64_t)N * OH * OW * (ST_KP / 4);
+    constexpr int K = 3 * KS * KS;
+    const int64_t total4 = (int64_t)N * OH * OW * (KP / 4);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += (int64_t)gridDim.x * blockDim.x) {
-        const int k4 = (int)(i % (ST_KP / 4));
-        const int64_t pix = i / (ST_KP / 4);
+        const int k4 = (int)(i % (KP / 4));
+        const int64_t pix = i / (KP / 4);
         const int ox = (int)(pix % OW), oy = (int)((pix / OW) % OH), n = (int)(pix / ((int64_t)OW * OH));
         float v[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
             const int k = k4 * 4 + e;
             float x = 0.f;
-            if (k < ST_K) {
-                const int c = k % 3, rs = k / 3, r = rs / 7, sx = rs - r * 7;
-                const int iy = oy * 2 - 3 + r, ix = ox * 2 - 3 + sx;
+            if (k < K) {
+                const int c = k % 3, rs = k / 3, r = rs / KS, sx = rs - r * KS;
+                const int iy = oy * 2 - PAD + r, ix = ox * 2 - PAD + sx;
                 if (iy >= 0 && iy < H && ix >= 0 && ix < W) x = __ldg(img + ((int64_t)(n * 3 + c) * H + iy) * W + ix);
             }
             v[e] = x;
@@ -637,41 +643,62 @@ stem_im2col_kernel(const float* __restrict__ img, float* __restrict__ cols, int 
     }
 }
 
-extern "C" int pxl_stem_im2col(const float* img, float* cols, int N, int H, int W, int OH, int OW, void* stream) {
+template <int KS, int PAD, int KP>
+static int stem_im2col_run(const float* img, float* cols, int N, int H, int W, int OH, int OW, void* stream) {
     if (!img || !cols || N <= 0 || H <= 0 || W <= 0 || OH <= 0 || OW <= 0) return PXL_ERR_BAD_ARG;
-    const int64_t total4 = (int64_t)N * OH * OW * (ST_KP / 4);
+    const int64_t total4 = (int64_t)N * OH * OW * (KP / 4);
     int64_t blocks = pxl_cdiv(total4, 256 * 4);
     if (blocks > PXL_NUM_SMS * 16) blocks = PXL_NUM_SMS * 16;
-    stem_im2col_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(img, cols, N, H, W, OH, OW);
+    stem_im2col_kernel<KS, PAD, KP><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(img, cols, N, H, W, OH, OW);
     PXL_CHECK_LAUNCH();
     return 0;
 }
 
+extern "C" int pxl_stem_im2col(const float* img, float* cols, int N, int H, int W, int OH, int OW, void* stream) {
+    return stem_im2col_run<7, 3, ST_KP>(img, cols, N, H, W, OH, OW, stream);
+}
+
+extern "C" int pxl_stem3x3s2_im2col(const float* img, float* cols, int N, int H, int W, int OH, int OW, void* stream) {
+    return stem_im2col_run<3, 1, ST3_KP>(img, cols, N, H, W, OH, OW, stream);
+}
+
 // fp16-pair variant for the f16 wgmma tensor-core path (csrc/h16_prep.cu): the unfolded stem matrix is written directly
-// as hi / lo planes [pixels][192] (147 taps*channels + 45 zero lanes: K must be a multiple of the 64-element operand
-// row), value * scale = hi + lo.  768 B per output pixel instead of 640 B of fp32, and no separate split pass.
+// as hi / lo planes [pixels][KH] (KH: the taps*channels rounded up to the 64-element operand row; 7x7: 147 + 45 zero
+// lanes = 192, 3x3: 27 + 37 = 64), value * scale = hi + lo.  For the 7x7 stem that is 768 B per output pixel instead of
+// 640 B of fp32, and no separate split pass.
 #include <cuda_fp16.h>
 #define ST_KH 192
+#define ST3_KH 64
 #define IM_TOX 32                       // output tile of a CTA: 32 x 4 pixels of one image
 #define IM_TOY 4
-#define IM_PW (2 * IM_TOX + 5)          // input patch it touches: 69 x 13 pixels x 3 channels (10.8 KB of shared memory)
-#define IM_PH (2 * IM_TOY + 5)
-__constant__ int c_im_koff[ST_KH];      // k -> offset of tap k inside the patch for the tile's first pixel (-1: zero lane)
+// input patch a tile touches: (2*32 + KS-2) x (2*4 + KS-2) pixels x 3 channels (7x7: 69 x 13, 10.8 KB of shared memory;
+// 3x3: 65 x 9, 7.0 KB)
+template <int KS> struct StemPatch {
+    static constexpr int PW = 2 * IM_TOX + KS - 2, PH = 2 * IM_TOY + KS - 2;
+};
+// k -> offset of tap k inside the patch for the tile's first pixel (-1: zero lane), one table per geometry
+__constant__ int c_im_koff[ST_KH];
+__constant__ int c_im3_koff[ST3_KH];
+template <int KS> __device__ __forceinline__ int stem_koff(int k);
+template <> __device__ __forceinline__ int stem_koff<7>(int k) { return c_im_koff[k]; }
+template <> __device__ __forceinline__ int stem_koff<3>(int k) { return c_im3_koff[k]; }
 
 // The patch is staged once in shared memory (coalesced rows, zero outside the image = the convolution's padding); every
-// thread then emits 4-lane groups of the [pixels][192] matrix with one table lookup + one shared-memory load per value
+// thread then emits 4-lane groups of the [pixels][KH] matrix with one table lookup + one shared-memory load per value
 // instead of a div/mod chain and a scattered global load (the round-2 first version: 0.71 ms per launch).
+template <int KS, int PAD, int KH>
 __global__ void __launch_bounds__(256)
 stem_im2col_h16_kernel(const float* __restrict__ img, uint2* __restrict__ hi, uint2* __restrict__ lo, float scale,
                        int N, int H, int W, int OH, int OW, int tilesX, int tilesY, int* __restrict__ sat) {
+    constexpr int IM_PW = StemPatch<KS>::PW, IM_PH = StemPatch<KS>::PH;
     __shared__ float patch[3 * IM_PH * IM_PW];
-    __shared__ short koff_s[ST_KH];          // the lanes of a warp index the table with 32 different k: from constant memory
+    __shared__ short koff_s[KH];             // the lanes of a warp index the table with 32 different k: from constant memory
                                              // that serialises 32-fold
-    for (int i = threadIdx.x; i < ST_KH; i += blockDim.x) koff_s[i] = (short)c_im_koff[i];
+    for (int i = threadIdx.x; i < KH; i += blockDim.x) koff_s[i] = (short)stem_koff<KS>(i);
     const int t = blockIdx.x;
     const int tx = t % tilesX, ty = (t / tilesX) % tilesY, n = t / (tilesX * tilesY);
     const int ox0 = tx * IM_TOX, oy0 = ty * IM_TOY;
-    const int ix0 = ox0 * 2 - 3, iy0 = oy0 * 2 - 3;
+    const int ix0 = ox0 * 2 - PAD, iy0 = oy0 * 2 - PAD;
     for (int i = threadIdx.x; i < 3 * IM_PH * IM_PW; i += blockDim.x) {
         const int px = i % IM_PW, py = (i / IM_PW) % IM_PH, c = i / (IM_PW * IM_PH);
         const int iy = iy0 + py, ix = ix0 + px;
@@ -679,8 +706,8 @@ stem_im2col_h16_kernel(const float* __restrict__ img, uint2* __restrict__ hi, ui
     }
     __syncthreads();
     bool clipped = false;
-    for (int i = threadIdx.x; i < IM_TOX * IM_TOY * (ST_KH / 4); i += blockDim.x) {
-        const int k4 = i % (ST_KH / 4), p = i / (ST_KH / 4);
+    for (int i = threadIdx.x; i < IM_TOX * IM_TOY * (KH / 4); i += blockDim.x) {
+        const int k4 = i % (KH / 4), p = i / (KH / 4);
         const int lx = p % IM_TOX, ly = p / IM_TOX;
         const int ox = ox0 + lx, oy = oy0 + ly;
         if (ox >= OW || oy >= OH) continue;
@@ -696,7 +723,7 @@ stem_im2col_h16_kernel(const float* __restrict__ img, uint2* __restrict__ hi, ui
             h[e] = __half_as_ushort(hh);
             l[e] = __half_as_ushort(__float2half_rn(cl - __half2float(hh)));
         }
-        const int64_t o = (((int64_t)n * OH + oy) * OW + ox) * (ST_KH / 4) + k4;
+        const int64_t o = (((int64_t)n * OH + oy) * OW + ox) * (KH / 4) + k4;
         hi[o] = make_uint2((uint32_t)h[0] | ((uint32_t)h[1] << 16), (uint32_t)h[2] | ((uint32_t)h[3] << 16));
         if (lo) lo[o] = make_uint2((uint32_t)l[0] | ((uint32_t)l[1] << 16), (uint32_t)l[2] | ((uint32_t)l[3] << 16));
     }
@@ -705,25 +732,39 @@ stem_im2col_h16_kernel(const float* __restrict__ img, uint2* __restrict__ hi, ui
 
 extern "C" int* pxl_h16_sat_counter(void);
 
-extern "C" int pxl_stem_im2col_h16(const float* img, void* hi, void* lo, float scale, int N, int H, int W, int OH, int OW,
-                                   void* stream) {
+// table: the geometry's constant-memory tap table, uploaded on the first call (the flag is per geometry)
+template <int KS, int PAD, int KH>
+static int stem_im2col_h16_run(const void* table, bool& uploaded, const float* img, void* hi, void* lo, float scale,
+                               int N, int H, int W, int OH, int OW, void* stream) {
     if (!img || !hi || !(scale > 0.f) || N <= 0 || H <= 0 || W <= 0 || OH <= 0 || OW <= 0) return PXL_ERR_BAD_ARG;
-    static bool table = false;
-    if (!table) {
-        int koff[ST_KH];
-        for (int k = 0; k < ST_KH; ++k) {
-            if (k >= ST_K) { koff[k] = -1; continue; }
-            const int c = k % 3, rs = k / 3, r = rs / 7, sx = rs - r * 7;
+    if (!uploaded) {
+        constexpr int IM_PW = StemPatch<KS>::PW, IM_PH = StemPatch<KS>::PH;
+        int koff[KH];
+        for (int k = 0; k < KH; ++k) {
+            if (k >= 3 * KS * KS) { koff[k] = -1; continue; }
+            const int c = k % 3, rs = k / 3, r = rs / KS, sx = rs - r * KS;
             koff[k] = (c * IM_PH + r) * IM_PW + sx;
         }
-        if (cudaMemcpyToSymbol(c_im_koff, koff, sizeof(koff)) != cudaSuccess) return PXL_ERR_BAD_ARG;
-        table = true;
+        if (cudaMemcpyToSymbol(table, koff, sizeof(koff)) != cudaSuccess) return PXL_ERR_BAD_ARG;
+        uploaded = true;
     }
     const int tilesX = (OW + IM_TOX - 1) / IM_TOX, tilesY = (OH + IM_TOY - 1) / IM_TOY;
     const int64_t blocks = (int64_t)N * tilesX * tilesY;
     if (blocks > 0x7fffffff) return PXL_ERR_UNSUPPORTED;
-    stem_im2col_h16_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(img, (uint2*)hi, (uint2*)lo, scale, N, H, W, OH, OW,
-                                                                              tilesX, tilesY, pxl_h16_sat_counter());
+    stem_im2col_h16_kernel<KS, PAD, KH><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+        img, (uint2*)hi, (uint2*)lo, scale, N, H, W, OH, OW, tilesX, tilesY, pxl_h16_sat_counter());
     PXL_CHECK_LAUNCH();
     return 0;
+}
+
+extern "C" int pxl_stem_im2col_h16(const float* img, void* hi, void* lo, float scale, int N, int H, int W, int OH, int OW,
+                                   void* stream) {
+    static bool uploaded = false;
+    return stem_im2col_h16_run<7, 3, ST_KH>(c_im_koff, uploaded, img, hi, lo, scale, N, H, W, OH, OW, stream);
+}
+
+extern "C" int pxl_stem3x3s2_im2col_h16(const float* img, void* hi, void* lo, float scale, int N, int H, int W, int OH,
+                                        int OW, void* stream) {
+    static bool uploaded = false;
+    return stem_im2col_h16_run<3, 1, ST3_KH>(c_im3_koff, uploaded, img, hi, lo, scale, N, H, W, OH, OW, stream);
 }

@@ -1129,75 +1129,89 @@ def aspp(x, weights, biases, dilations=(6, 12, 18, 24)):
     return _Aspp.apply(x, tuple(dilations), *(tuple(weights) + tuple(biases)))
 
 
-class _Stem(torch.autograd.Function):
-    """conv 7x7/2 pad 3 on the planar image -> NHWC (resnet.py:69,121); no input gradient.
+# stride-2 stem convolutions on the planar image, by kernel size: padding, then the fp32 and fp16-pair unfold entry points
+# with their matrix widths (the taps*channels rounded up to the tf32 / fp16 kernels' channel multiple of 32 / 64)
+STEM_GEOMETRIES = {
+    7: (3, ('pxl_stem_im2col', 160), ('pxl_stem_im2col_h16', 192)),              # ResNet's 7x7/2 pad 3, 3 -> 64
+    3: (1, ('pxl_stem3x3s2_im2col', 32), ('pxl_stem3x3s2_im2col_h16', 64)),      # the deep stem's first 3x3/2 pad 1
+}
 
-    fp32 mode: the dedicated FFMA kernels.  Tensor-core modes: the image is unfolded once into a
-    [pixels, 160] matrix (147 taps*channels + 13 zero lanes) and the stem runs as a flat 1x1 convolution on
-    wgmma, forward and wgrad sharing the matrix (19.9 GFLOP each on the 513x513 x16 batch)."""
+
+class _Stem(torch.autograd.Function):
+    """conv KxK/2 on the planar image -> NHWC, K in STEM_GEOMETRIES (resnet.py:69,121); no input gradient.
+
+    Tensor-core modes: the image is unfolded once into a [pixels, lanes] matrix (K*K*3 taps*channels + zero lanes) and
+    the stem runs as a flat 1x1 convolution on wgmma, forward and wgrad sharing the matrix (19.9 GFLOP each for the 7x7
+    stem on the 513x513 x16 batch).  fp32 mode: the 7x7 stem has dedicated FFMA kernels; the 3x3 one runs its fp32
+    matrix through the FFMA convolution kernels."""
 
     @staticmethod
-    def forward(ctx, img, weight, sums):
+    def forward(ctx, img, weight, sums, ks):
         _chk(img, 'img'); _chk(weight, 'weight', cl=True)
         N, C, H, W = img.shape
-        if C != 3 or tuple(weight.shape) != (64, 3, 7, 7):
-            raise ValueError('stem expects a 3-channel image and a [64,3,7,7] weight')
-        OH, OW = (H + 6 - 7) // 2 + 1, (W + 6 - 7) // 2 + 1
+        if ks not in STEM_GEOMETRIES or C != 3 or tuple(weight.shape) != (64, 3, ks, ks):
+            raise ValueError('stem expects a 3-channel image and a [64,3,7,7] or [64,3,3,3] weight')
+        pad, (fp32_entry, kp), (h16_entry, kh) = STEM_GEOMETRIES[ks]
+        K = 3 * ks * ks
+        OH, OW = (H + 2 * pad - ks) // 2 + 1, (W + 2 * pad - ks) // 2 + 1
         out = torch.empty((N, 64, OH, OW), dtype=torch.float32, device=img.device, memory_format=CL)
         prec = _conv_precision
-        ctx.meta = (N, H, W, OH, OW, prec)
-        if prec == 0:
+        ctx.meta = (N, H, W, OH, OW, prec, ks)
+        if prec == 0 and ks == 7:
             call('pxl_stem_conv7x7s2', _p(img), _p(weight), _p(out), N, H, W, OH, OW, _stream())
             ctx.save_for_backward(img)
             return out
         if prec >= 3:
-            # fp16-pair path: the unfolded matrix is written directly as the hi / lo planes [pixels][192]
+            # fp16-pair path: the unfolded matrix is written directly as the hi / lo planes [pixels][kh]
             want_lo = prec == 3
-            n = N * OH * OW * 192
+            n = N * OH * OW * kh
             buf = torch.empty((2, n), dtype=torch.float16, device=img.device)
-            call('pxl_stem_im2col_h16', _p(img), _p(buf[0]), _p(buf[1] if want_lo else None), float(H16_ACT_SCALE),
-                 N, H, W, OH, OW, _stream())
+            _timed_call(h16_entry, _p(img), _p(buf[0]), _p(buf[1] if want_lo else None), float(H16_ACT_SCALE),
+                        N, H, W, OH, OW, _stream())
             colsh = H16(buf, n, H16_ACT_SCALE, None, want_lo)
-            wp = torch.zeros((64, 192), dtype=torch.float32, device=img.device)
-            wp[:, :147] = weight.detach().permute(0, 2, 3, 1).reshape(64, 147)
-            conv_raw(colsh, h16_split(wp, H16_W_SCALE, want_lo), None, [0, 0], N, OH, OW, 192, OH, OW, 64, 64, 1, 1, out=out,
+            wp = torch.zeros((64, kh), dtype=torch.float32, device=img.device)
+            wp[:, :K] = weight.detach().permute(0, 2, 3, 1).reshape(64, K)
+            conv_raw(colsh, h16_split(wp, H16_W_SCALE, want_lo), None, [0, 0], N, OH, OW, kh, OH, OW, 64, 64, 1, 1, out=out,
                      precision=prec, bn_stats=sums)
             ctx.save_for_backward(buf if ctx.needs_input_grad[1] else None)
             ctx.h16 = want_lo
             return out
-        cols = torch.empty((N, 160, OH, OW), dtype=torch.float32, device=img.device, memory_format=CL)
-        call('pxl_stem_im2col', _p(img), _p(cols), N, H, W, OH, OW, _stream())
-        wp = torch.zeros((64, 160), dtype=torch.float32, device=img.device)
-        wp[:, :147] = weight.detach().permute(0, 2, 3, 1).reshape(64, 147)      # physical order of the CL weight
-        conv_raw(cols, wp, None, [0, 0], N, OH, OW, 160, OH, OW, 64, 64, 1, 1, out=out, precision=prec, bn_stats=sums)
+        cols = torch.empty((N, kp, OH, OW), dtype=torch.float32, device=img.device, memory_format=CL)
+        _timed_call(fp32_entry, _p(img), _p(cols), N, H, W, OH, OW, _stream())
+        wp = torch.zeros((64, kp), dtype=torch.float32, device=img.device)
+        wp[:, :K] = weight.detach().permute(0, 2, 3, 1).reshape(64, K)          # physical order of the CL weight
+        conv_raw(cols, wp, None, [0, 0], N, OH, OW, kp, OH, OW, 64, 64, 1, 1, out=out, precision=prec, bn_stats=sums)
         ctx.save_for_backward(cols if ctx.needs_input_grad[1] else None)
         return out
 
     @staticmethod
     def backward(ctx, dy):
         (saved,) = ctx.saved_tensors
-        N, H, W, OH, OW, prec = ctx.meta
+        N, H, W, OH, OW, prec, ks = ctx.meta
+        pad, (_, kp), (_, kh) = STEM_GEOMETRIES[ks]
+        K = 3 * ks * ks
         dy = as_cl(dy)
-        if prec == 0:
+        if prec == 0 and ks == 7:
             dw = torch.empty((64, 3, 7, 7), dtype=torch.float32, device=dy.device, memory_format=CL).zero_()
             call('pxl_stem_conv7x7s2_wgrad', _p(saved), _p(dy), _p(dw), N, H, W, OH, OW, _stream())
-            return None, dw, None
+            return None, dw, None, None
         if prec >= 3:
-            dwp = torch.zeros((64, 192), dtype=torch.float32, device=dy.device)
-            conv_wgrad_raw(H16(saved, saved.shape[1], H16_ACT_SCALE, None, ctx.h16), dy, dwp, [0, 0], N, OH, OW, 192, OH, OW, 64, 64,
+            dwp = torch.zeros((64, kh), dtype=torch.float32, device=dy.device)
+            conv_wgrad_raw(H16(saved, saved.shape[1], H16_ACT_SCALE, None, ctx.h16), dy, dwp, [0, 0], N, OH, OW, kh, OH, OW, 64, 64,
                            1, 1, precision=prec)
-            dw = dwp[:, :147].reshape(64, 7, 7, 3).permute(0, 3, 1, 2)
-            return None, dw, None
-        dwp = torch.zeros((64, 160), dtype=torch.float32, device=dy.device)
-        conv_wgrad_raw(saved, dy, dwp, [0, 0], N, OH, OW, 160, OH, OW, 64, 64, 1, 1, precision=prec)
-        dw = dwp[:, :147].reshape(64, 7, 7, 3).permute(0, 3, 1, 2)              # logical [64,3,7,7], CL strides
-        return None, dw, None
+        else:
+            dwp = torch.zeros((64, kp), dtype=torch.float32, device=dy.device)
+            conv_wgrad_raw(saved, dy, dwp, [0, 0], N, OH, OW, kp, OH, OW, 64, 64, 1, 1, precision=prec)
+        dw = dwp[:, :K].reshape(64, ks, ks, 3).permute(0, 3, 1, 2)              # logical [64,3,ks,ks], CL strides
+        return None, dw, None, None
 
 
 def stem_conv(img, weight, want_bn_stats=False):
-    """want_bn_stats: like conv2d - on the tensor-core path the epilogue accumulates the BN sums."""
+    """The stride-2 stem convolution (64 output channels) whose geometry the weight's kernel size selects: ResNet's
+    7x7 pad 3 or the deep stem's first 3x3 pad 1.  want_bn_stats: like conv2d - on the tensor-core path the epilogue
+    accumulates the BN sums."""
     sums = _stat_zeros(128, img.device) if (want_bn_stats and _conv_precision != 0) else None
-    out = _Stem.apply(img.contiguous(), weight, sums)
+    out = _Stem.apply(img.contiguous(), weight, sums, int(weight.shape[-1]))
     if sums is not None and getattr(sums, '_pxl_filled', False):
         out._pxl_bn_sums = sums
     return out

@@ -9,6 +9,7 @@ from ... import ops
 from ...utils import logger, cmd
 from . import evaluation
 from .module import deeplab_v2, deeplab_v3plus, pspnet as pspnet_module
+from .module.resnet import BACKBONES
 
 
 def add_parser_arguments(parser):
@@ -16,8 +17,9 @@ def add_parser_arguments(parser):
     parser.add_argument('--backbone', type=str, default='resnet101')
     parser.add_argument('--freeze-bn', type=cmd.str2bool, default=False)
     # 'auto' = the URL the reference hard-codes for args.backbone (task/sseg/model.py:69-80), served from the local
-    # torch-hub cache / $PXL_PRETRAINED_DIR when present, downloaded otherwise; 'none' = keep the reference
-    # initialisers; anything else = a local file or URL.  A requested-but-unloadable backbone is an error.
+    # torch-hub cache / $PXL_PRETRAINED_DIR when present, downloaded otherwise (the *-deepstem backbones have none);
+    # 'none' = keep the reference initialisers; anything else = a local file or URL.  A requested-but-unloadable
+    # backbone is an error.
     parser.add_argument('--pretrained-backbone', type=str, default='auto')
 
 
@@ -80,6 +82,10 @@ def pretrained_backbone_url(args):
     if want in (None, '', 'none', 'None', False):
         return None
     if want == 'auto':
+        if args.backbone.endswith('-deepstem'):
+            logger.log_err('--pretrained-backbone auto has no download for the backbone {0}: pass the local file of its '
+                           'ImageNet weights (CPS resnet101_v1c.pth / UniMatch pretrained/resnet101.pth layout) or '
+                           'none\n'.format(args.backbone))
         return PRETRAINED_BACKBONE_URLS.get(args.backbone)
     return want
 
@@ -89,7 +95,7 @@ class DeepLabV2(TaskModel):
 
     def __init__(self, args):
         super().__init__(args)
-        if args.backbone not in ('resnet50', 'resnet101', 'resnet101-coco'):
+        if args.backbone not in BACKBONES:
             logger.log_err('{0} does not support the backbone: {1}\n'.format(type(self).__name__, args.backbone))
         self.model = self.MODULE(backbone=args.backbone, output_stride=args.output_stride, num_classes=args.num_classes,
                                  sync_bn=True, freeze_bn=args.freeze_bn,
@@ -143,7 +149,7 @@ class PSPNet(TaskModel):
 
     def __init__(self, args):
         super().__init__(args)
-        if args.backbone not in ('resnet50', 'resnet101', 'resnet101-coco'):
+        if args.backbone not in BACKBONES:
             logger.log_err('PSPNet does not support the backbone: {0}\n'.format(args.backbone))
         self.model = pspnet_module.PSPNet(backbone=args.backbone, output_stride=args.output_stride,
                                           num_classes=args.num_classes, sync_bn=True, freeze_bn=args.freeze_bn,
