@@ -532,6 +532,21 @@ int pxl_eval_view_add(const float* P, float* S, int n, int C, int hv, int wv, in
                       void* stream);
 int pxl_eval_finish(const float* S, float* mean, float* logmean, int64_t count, int V, void* stream);
 
+/* Depthwise 3x3 convolution (groups = C, bias-free; csrc/depthwise.cu), FFMA fp32 in every precision mode.
+ * Activations NHWC fp32 with ld lanes (C <= ld, C % 4 == 0, ld % 4 == 0, 16-byte aligned); w [C][9] (tap r*3 + s of
+ * the logical [C,1,3,3] weight).  Stride 1 with dilation >= 1, or stride 2 with dilation 1 (else PXL_ERR_UNSUPPORTED);
+ * padding = dilation, so OH = (H - 1) / stride + 1, OW likewise.  Output lanes c >= C are written 0.
+ * pxl_dw_conv_fwd:   y [N,OH,OW,ld] = conv(x [N,H,W,ld]).
+ * pxl_dw_conv_dgrad: dx [N,H,W,ld] from dy [N,OH,OW,ld] (a gather; stride 2 by output parity).
+ * pxl_dw_conv_wgrad: dw [C][9] (accumulate: +=) = sum over the batch of x * dy; per-block fp64 partials in a
+ *   per-stream workspace, added in a fixed order by a second launch (no floating-point atomics). */
+int pxl_dw_conv_fwd(const float* x, const float* w, float* y, int N, int H, int W, int C, int ld, int OH, int OW,
+                    int stride, int dilation, void* stream);
+int pxl_dw_conv_dgrad(const float* dy, const float* w, float* dx, int N, int H, int W, int C, int ld, int OH, int OW,
+                      int stride, int dilation, void* stream);
+int pxl_dw_conv_wgrad(const float* x, const float* dy, float* dw, int N, int H, int W, int C, int ld, int OH, int OW,
+                      int stride, int dilation, int accumulate, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -139,6 +139,9 @@ SIGNATURES = {
                                c_int, P, P]),
     'pxl_eval_view_add': (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
     'pxl_eval_finish': (c_int, [P, P, P, c_int64, c_int, P]),
+    'pxl_dw_conv_fwd': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
+    'pxl_dw_conv_dgrad': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
+    'pxl_dw_conv_wgrad': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P]),
 }
 
 PXL_ERR_BAD_ARG = -1

@@ -10,7 +10,7 @@ LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'libpixelssl_b200.so')
 SOURCES = ['loss_kernels.cu', 'norm_pool_optim.cu', 'resample.cu', 'conv_fp32.cu', 'conv_tc.cu',
            'h16_prep.cu', 'conv_api.cu', 'gct_kernels.cu', 'metrics_noise.cu', 'peer_exchange.cu', 'input_pipeline.cu', 'aspp_gather.cu', 's4l_kernels.cu',
-           'lane_concat.cu', 'strong_aug.cu', 'ohem.cu', 'eval_views.cu']
+           'lane_concat.cu', 'strong_aug.cu', 'ohem.cu', 'eval_views.cu', 'depthwise.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '--use_fast_math=false']
 

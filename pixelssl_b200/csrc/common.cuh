@@ -16,7 +16,8 @@ extern "C" void pxl_count_launch_(int n);
 #define PXL_WS_UNIMATCH 4
 #define PXL_WS_STRONG_AUG 5
 #define PXL_WS_OHEM 6
-#define PXL_WS_PURPOSES 7
+#define PXL_WS_DEPTHWISE 7
+#define PXL_WS_PURPOSES 8
 #define PXL_WS_STREAMS 8
 extern "C" void* pxl_workspace_(int purpose, void* stream, size_t bytes, int* rc);
 

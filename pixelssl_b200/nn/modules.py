@@ -45,6 +45,26 @@ class Conv2d(nn.Module):
                'dilation={dilation}'.format(**self.__dict__)
 
 
+class DepthwiseConv2d(nn.Module):
+    """nn.Conv2d(channels, channels, 3, stride, padding=dilation, dilation=dilation, groups=channels, bias=False)
+    replacement: weight [C,1,3,3] (contiguous = [C][9], the layout the depthwise kernels read)."""
+
+    def __init__(self, channels, stride=1, dilation=1):
+        super().__init__()
+        self.in_channels = self.out_channels = channels
+        self.kernel_size = (3, 3)
+        self.stride, self.dilation, self.padding = stride, dilation, dilation
+        w = torch.empty(channels, 1, 3, 3)
+        nn.init.kaiming_uniform_(w, a=math.sqrt(5))        # nn.Conv2d default
+        self.weight = nn.Parameter(w)
+
+    def forward(self, x):
+        return ops.depthwise_conv(ops.as_cl(x), self.weight, self.stride, self.dilation)
+
+    def extra_repr(self):
+        return '{in_channels}, stride={stride}, dilation={dilation}'.format(**self.__dict__)
+
+
 class BatchNorm2d(nn.Module):
     """SynchronizedBatchNorm2d of the reference (sync_batchnorm/batchnorm.py:180): momentum 0.1,
     eps 1e-5, affine.  ``forward(x, relu=False, residual=None)`` fuses what follows the BN in

@@ -1523,6 +1523,125 @@ def conv_bn_act(x, conv, bn, relu=False, residual=None, out_mode='both', stash_k
     return out
 
 
+# ------------------------------------------------------------------------------------------------
+# depthwise 3x3 convolution: the per-channel half of a separable convolution (csrc/depthwise.cu)
+# ------------------------------------------------------------------------------------------------
+
+def _dw_geometry(x, weight, stride, dilation):
+    _chk(x, 'x', cl=True); _chk(weight, 'weight')
+    N, ld, H, W = x.shape
+    C = weight.shape[0]
+    if tuple(weight.shape) != (C, 1, 3, 3) or C > ld:
+        raise ValueError('depthwise weight must be [C,1,3,3] with C <= the input lanes (got %s for %d lanes)'
+                         % (tuple(weight.shape), ld))
+    return N, ld, H, W, C, (H - 1) // stride + 1, (W - 1) // stride + 1
+
+
+def _dw_backward(x, weight, dy, meta, want_dx, want_dw):
+    """-> (dx, dw) of the depthwise convolution; dw is None when it was added straight into weight.grad."""
+    N, ld, H, W, C, OH, OW, stride, dilation = meta
+    dx = dw = None
+    moved = 4 * N * ld * (H * W + OH * OW)
+    if want_dx:
+        dx = torch.empty_like(x)
+        _timed_call('pxl_dw_conv_dgrad', _p(dy), _p(weight), _p(dx), N, H, W, C, ld, OH, OW, stride, dilation, _stream(),
+                    meta=(moved, 'dgrad N%d %dx%d C%d ld%d s%d d%d' % (N, H, W, C, ld, stride, dilation)))
+    if want_dw:
+        inplace = weight.grad is not None and weight.grad.is_contiguous()
+        dwbuf = weight.grad if inplace else torch.empty_like(weight)
+        _timed_call('pxl_dw_conv_wgrad', _p(x), _p(dy), _p(dwbuf), N, H, W, C, ld, OH, OW, stride, dilation,
+                    1 if inplace else 0, _stream(),
+                    meta=(moved, 'wgrad N%d %dx%d C%d ld%d s%d d%d' % (N, H, W, C, ld, stride, dilation)))
+        dw = None if inplace else dwbuf
+    return dx, dw
+
+
+def _dw_forward(x, weight, stride, dilation):
+    N, ld, H, W, C, OH, OW = _dw_geometry(x, weight, stride, dilation)
+    y = torch.empty((N, ld, OH, OW), dtype=torch.float32, device=x.device, memory_format=CL)
+    _timed_call('pxl_dw_conv_fwd', _p(x), _p(weight), _p(y), N, H, W, C, ld, OH, OW, stride, dilation, _stream(),
+                meta=(4 * N * ld * (H * W + OH * OW), 'fwd N%d %dx%d C%d ld%d s%d d%d' % (N, H, W, C, ld, stride, dilation)))
+    return y, (N, ld, H, W, C, OH, OW, stride, dilation)
+
+
+class _DepthwiseConv(torch.autograd.Function):
+    """nn.Conv2d(C, C, 3, stride, padding=dilation, dilation=dilation, groups=C, bias=False) on an NHWC tensor with
+    ld >= C lanes; lanes >= C of the output are zero.  FFMA fp32 in every precision mode (it is bandwidth-bound, so the
+    tensor cores would buy nothing); it never goes through conv_route."""
+
+    @staticmethod
+    def forward(ctx, x, weight, stride, dilation):
+        y, ctx.meta = _dw_forward(x, weight, stride, dilation)
+        ctx.save_for_backward(x, weight)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight = ctx.saved_tensors
+        dx, dw = _dw_backward(x, weight, as_cl(dy), ctx.meta, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        return dx, dw, None, None
+
+
+def depthwise_conv(x, weight, stride=1, dilation=1):
+    """Depthwise 3x3 convolution, padding = dilation (Xception's fixed_padding): weight [C,1,3,3] contiguous, x NHWC
+    with C <= lanes; stride 1 with any dilation or stride 2 with dilation 1."""
+    return _DepthwiseConv.apply(x, weight, int(stride), int(dilation))
+
+
+class _DwBnPair(torch.autograd.Function):
+    """Depthwise convolution -> train-mode (Sync)BN as one node whose output is only the fp16 pair the pointwise
+    convolution's _ConvBnAct unit reads (an ``out_mode='pair'`` carrier): the BN apply launch writes the pair, so the
+    normalised depthwise output never exists in fp32.  The statistics come from the BN statistics pass over the
+    depthwise output.  Backward: the BN backward (fp32), then the depthwise dgrad and wgrad."""
+
+    @staticmethod
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, stride, dilation, momentum, eps, group, clamp_var):
+        global _unit_out_pair
+        want_lo = _conv_precision == 3
+        c, meta = _dw_forward(x, weight, stride, dilation)
+        N, ld, H, W, C, OH, OW = meta[:7]
+        rows, dev = N * OH * OW, x.device
+        n = rows * ld
+        sums = _stat_zeros(2 * ld, dev)
+        call('pxl_bn_stats', _p(c), rows, ld, _p(sums), _stream())
+        coeff = torch.empty((4, ld), dtype=torch.float32, device=dev)
+        pair = torch.empty((2, n), dtype=torch.float16, device=dev)
+        count = _bn_train_forward(c, sums, rows, ld, gamma, beta, running_mean, running_var, momentum, eps, clamp_var,
+                                  group, coeff, None, False, None,
+                                  (_p(pair[0]), _p(pair[1] if want_lo else None), float(H16_ACT_SCALE), None))
+        ctx.save_for_backward(x, weight, c, gamma, coeff, beta)
+        ctx.meta, ctx.bn = meta, (count, group)
+        _unit_out_pair = H16(pair, n, H16_ACT_SCALE, None, want_lo)
+        return pair.view(torch.float32).view(N, OH, OW, ld).permute(0, 3, 1, 2)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight, c, gamma, coeff, beta = ctx.saved_tensors
+        count, group = ctx.bn
+        N, ld, H, W, C, OH, OW = ctx.meta[:7]
+        dy = as_cl(dy)
+        rows, dev = N * OH * OW, dy.device
+        dsums = _stat_zeros(2 * ld, dev)
+        call('pxl_bn_bwd_reduce', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), 0, rows, ld, _p(dsums),
+             _p(coeff[2]), _p(coeff[3]), _stream())
+        dgamma, dbeta, gacc, bacc = _bn_backward_sums(dsums, ld, gamma, beta, group)
+        dc = torch.empty_like(c)
+        call('pxl_bn_bwd_dx', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, 0,
+             _p(dc), None, rows, ld, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc), _stream())
+        dx, dw = _dw_backward(x, weight, dc, ctx.meta, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        return (dx, dw, dgamma, dbeta) + (None,) * 8
+
+
+def depthwise_bn_pair(x, weight, bn, stride=1, dilation=1):
+    """depthwise_conv -> bn (train mode, the BatchNorm2d or a lane-padded view of it with the same attributes) as the
+    fp16-pair carrier a following conv_bn_act unit reads; see _DwBnPair."""
+    global _unit_out_pair
+    out = _DwBnPair.apply(x, weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, int(stride), int(dilation),
+                          float(bn.momentum), float(bn.eps), bn.sync_group, bool(bn.multi_replica_formula))
+    pair, _unit_out_pair = _unit_out_pair, None
+    return _attach_pair(out, pair, carrier=True)
+
+
 class _MaxPool(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x):

@@ -17,7 +17,8 @@ def add_parser_arguments(parser):
     parser.add_argument('--backbone', type=str, default='resnet101')
     parser.add_argument('--freeze-bn', type=cmd.str2bool, default=False)
     # 'auto' = the URL the reference hard-codes for args.backbone (task/sseg/model.py:69-80), served from the local
-    # torch-hub cache / $PXL_PRETRAINED_DIR when present, downloaded otherwise (the *-deepstem backbones have none);
+    # torch-hub cache / $PXL_PRETRAINED_DIR when present, downloaded otherwise (the *-deepstem backbones and xception65
+    # have none);
     # 'none' = keep the reference initialisers; anything else = a local file or URL.  A requested-but-unloadable
     # backbone is an error.
     parser.add_argument('--pretrained-backbone', type=str, default='auto')
@@ -82,6 +83,10 @@ def pretrained_backbone_url(args):
     if want in (None, '', 'none', 'None', False):
         return None
     if want == 'auto':
+        if args.backbone == 'xception65':
+            logger.log_err('--pretrained-backbone auto has no download for the backbone xception65: pass the local file '
+                           'of its ImageNet weights (in the key layout of the aligned Xception-65 module tree) or '
+                           'none\n')
         if args.backbone.endswith('-deepstem'):
             logger.log_err('--pretrained-backbone auto has no download for the backbone {0}: pass the local file of its '
                            'ImageNet weights (CPS resnet101_v1c.pth / UniMatch pretrained/resnet101.pth layout) or '
@@ -92,10 +97,11 @@ def pretrained_backbone_url(args):
 
 class DeepLabV2(TaskModel):
     MODULE = deeplab_v2.DeepLabV2
+    BACKBONES = tuple(BACKBONES)
 
     def __init__(self, args):
         super().__init__(args)
-        if args.backbone not in BACKBONES:
+        if args.backbone not in self.BACKBONES:
             logger.log_err('{0} does not support the backbone: {1}\n'.format(type(self).__name__, args.backbone))
         self.model = self.MODULE(backbone=args.backbone, output_stride=args.output_stride, num_classes=args.num_classes,
                                  sync_bn=True, freeze_bn=args.freeze_bn,
@@ -140,8 +146,9 @@ class DeepLabV2(TaskModel):
 
 class DeepLabV3Plus(DeepLabV2):
     """DeepLabV3+ with the DeepLabV2 plugin surface: same backbones, resulter keys and latent (the layer4 output);
-    backbone at 1x lr, ASPP, decoder and classifier at 10x."""
+    backbone at 1x lr, ASPP, decoder and classifier at 10x.  It also takes the aligned Xception-65 backbone."""
     MODULE = deeplab_v3plus.DeepLabV3Plus
+    BACKBONES = tuple(BACKBONES) + ('xception65',)
 
 
 class PSPNet(TaskModel):

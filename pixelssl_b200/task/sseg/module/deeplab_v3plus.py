@@ -1,11 +1,11 @@
-"""DeepLabV3+ (Chen et al., ECCV 2018) on the H100 kernels: the dilated ResNet backbone -> ASPP with image pooling
+"""DeepLabV3+ (Chen et al., ECCV 2018) on the H100 kernels: the dilated ResNet or aligned Xception-65 backbone -> ASPP with image pooling
 (parameter layout of torchvision.models.segmentation.deeplabv3.ASPP, without its dropout) -> decoder on the
 stride-4 low-level features -> 1x1 classifier -> bilinear (align_corners=True) to the input size.
 
 Every convolution runs on the library's convolution kernels.  The two concatenations are single launches of
 ``ops.lane_concat`` whose backward gathers in a fixed order.  Two shapes are padded so that the wgmma kernels
 (Cin % 64 == 0 on the fp16-pair path) take every head convolution in the tensor-core modes:
-  * ``decoder.reduce`` (256 -> 48) runs as 256 -> 64 with 16 zero output channels (zero weight rows, zero BN affine);
+  * ``decoder.reduce`` (256 -> 48, or 128 -> 48 on Xception-65) runs as 256 -> 64 with 16 zero output channels (zero weight rows, zero BN affine);
   * the decoder concat holds 256 + 48 channels in 320 lanes, and ``decoder.fuse.0``'s [256, 304, 3, 3] weight is
     zero-padded to 320 input channels at use.
 The checkpoint shapes stay the unpadded ones."""
@@ -18,6 +18,7 @@ import torch.nn.functional as F
 from .... import ops
 from ....nn.modules import Conv2d, BatchNorm2d
 from .resnet import build_backbone
+from .xception import AlignedXception
 
 ASPP_RATES = {16: (6, 12, 18), 8: (12, 24, 36)}
 DECODER_LANES = 320          # 256 upsampled ASPP channels + 48 reduced low-level channels, rounded up to 64
@@ -127,9 +128,13 @@ class DeepLabV3Plus(nn.Module):
                  pretrained_backbone_url=None):
         super().__init__()
         self.num_classes = num_classes
-        self.backbone = build_backbone(backbone, output_stride, pretrained_backbone_url)
+        if backbone == 'xception65':
+            self.backbone = AlignedXception(output_stride, pretrained_backbone_url)
+            self.FP_CHANNELS = (128, 2048)         # block1's (ReLU'd) output is the low-level feature
+        else:
+            self.backbone = build_backbone(backbone, output_stride, pretrained_backbone_url)
         self.aspp = ASPP(2048, ASPP_RATES[output_stride], 256)
-        self.decoder = Decoder(256, 256, 48, 256)
+        self.decoder = Decoder(self.FP_CHANNELS[0], 256, 48, 256)
         self.classifier = Conv2d(256, num_classes, 1, bias=True, out_lanes=(num_classes + 31) // 32 * 32)
         for m in list(self.aspp.modules()) + list(self.decoder.modules()):
             if isinstance(m, Conv2d):
@@ -152,7 +157,7 @@ class DeepLabV3Plus(nn.Module):
         return x, bx
 
     # the feature maps forward_fp perturbs, in the order of its ``scales``: layer1 (the decoder's low-level input) and
-    # layer4 (the ASPP input), as UniMatch drops both
+    # layer4 (the ASPP input), as UniMatch drops both; (128, 2048) on Xception-65
     FP_CHANNELS = (256, 2048)
 
     def forward_fp(self, img, scales):

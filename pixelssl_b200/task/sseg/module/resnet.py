@@ -146,19 +146,7 @@ class ResNet(nn.Module):
         statistic of the backbone must be present with its exact shape, so a 7x7-stem file fails instead of loading
         partially."""
         if self.deep_stem:
-            pre = torch.load(url, map_location='cpu') if os.path.isfile(url) else load_zoo_state_dict(url)
-            pre = {(k[len('module.'):] if k.startswith('module.') else k): v for k, v in pre.items()}
-            own = self.state_dict()
-            for k, v in own.items():
-                if k.endswith('.num_batches_tracked') and k not in pre:
-                    continue
-                if k not in pre:
-                    logger.log_err('pretrained backbone {0} has no key {1} (a deep-stem backbone needs every parameter and '
-                                   'BN running statistic of the network)\n'.format(url, k))
-                if tuple(pre[k].shape) != tuple(v.shape):
-                    logger.log_err('pretrained backbone {0}: key {1} has shape {2}, the deep-stem backbone needs {3}\n'
-                                   .format(url, k, tuple(pre[k].shape), tuple(v.shape)))
-            self.load_state_dict({k: pre.get(k, v) for k, v in own.items()})
+            load_complete_state_dict(self, url, 'deep-stem')
             return
         if os.path.isfile(url):
             self.load_state_dict(torch.load(url, map_location='cpu'))
@@ -189,6 +177,25 @@ def torchvision_dilation_plan(layers, output_stride):
         else:
             plan.append((2, [dilation] * n))
     return plan
+
+
+def load_complete_state_dict(module, url, kind):
+    """Load a local file (or zoo URL) that must hold every parameter and BN running statistic of ``module`` with its
+    exact shape: an optional ``module.`` prefix is stripped and keys the module does not have (``fc.*``) are dropped;
+    a missing or misshapen key stops the load and is named."""
+    pre = torch.load(url, map_location='cpu') if os.path.isfile(url) else load_zoo_state_dict(url)
+    pre = {(k[len('module.'):] if k.startswith('module.') else k): v for k, v in pre.items()}
+    own = module.state_dict()
+    for k, v in own.items():
+        if k.endswith('.num_batches_tracked') and k not in pre:
+            continue
+        if k not in pre:
+            logger.log_err('pretrained backbone {0} has no key {1} (a {2} backbone needs every parameter and '
+                           'BN running statistic of the network)\n'.format(url, k, kind))
+        if tuple(pre[k].shape) != tuple(v.shape):
+            logger.log_err('pretrained backbone {0}: key {1} has shape {2}, the {3} backbone needs {4}\n'
+                           .format(url, k, tuple(pre[k].shape), kind, tuple(v.shape)))
+    module.load_state_dict({k: pre.get(k, v) for k, v in own.items()})
 
 
 def load_zoo_state_dict(url):
