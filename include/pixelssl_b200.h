@@ -8,8 +8,9 @@
  * Each group cites the reference call site it replaces (paths relative to the PixelSSL tree).
  * Layouts: "NHWC" = channels innermost (torch channels_last), used for backbone activations;
  * "planar" = NCHW, used for the C=21 logit / probability maps exactly like the reference.
- * The reference-side binding is Python: see INTEGRATION.md (ctypes stub used by
- * pixelssl_b200/_lib.py).
+ * The reference-side binding is Python: pixelssl_b200/_lib.py reads the ctypes signatures from the
+ * pxl_* declarations of this file, so parameters and return values are pointers, int, int64_t, float
+ * or double (and void returns); see INTEGRATION.md.
  */
 #ifndef PIXELSSL_B200_H
 #define PIXELSSL_B200_H
@@ -162,6 +163,24 @@ int pxl_cutmix_confidence(const float* prob, int n, int C, int64_t HW, float thr
  *   running stats with the unbiased variance (momentum), writes scale=gamma*invstd,
  *   shift=beta-mean*scale.
  * apply: y = x*scale + shift (+ residual) (ReLU if relu!=0).
+ * backward of y = relu?(bn(x) + residual?):
+ *   reduce: dsums[0:C] = sum dz, dsums[C:2C] = sum dz*xhat with dz = dy * (y>0 if relu) (fp64;
+ *   caller zeroes; all-reduced for N>1);  writes nothing else.
+ *   dx:  dx = gamma*invstd*(dz - dsums0/count - xhat*dsums1/count); dres (nullable) = dz.
+ *   dgamma += dsums1, dbeta += dsums0 are produced by pxl_bn_bwd_params, or by the dx launch itself:
+ *   dgamma_acc / dbeta_acc (both or neither): dgamma_acc[c] += dsums[C+c], dbeta_acc[c] += dsums[c] (single-GPU
+ *   path: dsums are the local sums; replaces pxl_bn_bwd_params + the optimizer-side accumulation).
+ *   ReLU mask source, in this order: relu_mask, y, else recomputed as fmaf(x, scale, shift) > 0 (exactly what the
+ *   apply evaluated; only valid without a residual) - saves reading y.
+ * fp16 pairs (csrc/h16_prep.cu): the SAME pass that writes y (dx) also writes it as the fp16 pair the next wgmma
+ *   convolution reads, so the pair costs no extra trip through HBM.  hi / lo (dhi / dlo): __half NHWC planes, lo
+ *   nullable; hi NULL: no pair.  y (dx) may be NULL only when hi (dhi) is set: either the result or its pair is
+ *   written.  Forward: fixed scale `hscale`.  Backward: the reduce launch leaves absmax(dz) in amax_slot[2]
+ *   (nullable DEVICE float[4], zeroed), the dx launch derives the power-of-two scale from it, max|gamma*invstd| and
+ *   target_log2, and stores s / 1/s in slot[0] / slot[1] (slot required with dhi).
+ * relu_mask (nullable, rows*C/4 bytes): the forward launches store the sign bits of the result (bit k of byte i =
+ *   element 4i+k > 0); the backward launches then take the ReLU mask from it instead of re-reading the fp32 result
+ *   (0.25 B/element instead of 4).
  * ------------------------------------------------------------------------------------------- */
 int pxl_bn_stats(const float* x, int64_t rows, int C, double* sums, void* stream);
 int pxl_bn_finalize(const double* sums, double count, int C, const float* gamma, const float* beta,
@@ -171,51 +190,21 @@ int pxl_bn_finalize(const double* sums, double count, int C, const float* gamma,
 /* eval mode: scale/shift from running stats */
 int pxl_bn_eval_coeffs(int C, const float* gamma, const float* beta, const float* running_mean,
                        const float* running_var, float eps, float* scale, float* shift, void* stream);
-int pxl_bn_apply(const float* x, const float* scale, const float* shift, const float* residual,
-                 int relu, float* y, int64_t rows, int C, void* stream);
+int pxl_bn_apply(const float* x, const float* scale, const float* shift, const float* residual, int relu, float* y,
+                 int64_t rows, int C, void* hi, void* lo, float hscale, void* relu_mask, void* stream);
 /* training forward in one launch: pxl_bn_finalize + pxl_bn_apply (sums already hold the batch totals). */
-int pxl_bn_finalize_apply(const float* x, const double* sums, double count, const float* gamma,
-                          const float* beta, float* running_mean, float* running_var, float momentum,
-                          float eps, int clamp_mode, float* mean, float* invstd, float* scale, float* shift,
-                          const float* residual, int relu, float* y, int64_t rows, int C, void* stream);
-/* backward of y = relu?(bn(x) + residual?):
- *   reduce: dsums[0:C] = sum dz, dsums[C:2C] = sum dz*xhat with dz = dy * (y>0 if relu) (fp64;
- *   caller zeroes; all-reduced for N>1);  writes nothing else.
- *   dx:  dx = gamma*invstd*(dz - dsums0/count - xhat*dsums1/count); dres (nullable) = dz.
- *   dgamma += dsums1, dbeta += dsums0 are produced by pxl_bn_bwd_params.
- *   relu with y == NULL: the mask is recomputed as fmaf(x, scale, shift) > 0 (exactly what pxl_bn_apply
- *   evaluated; only valid without a residual) - saves reading y. */
-int pxl_bn_bwd_reduce(const float* x, const float* y, const float* dy, const float* mean,
-                      const float* invstd, int relu, int64_t rows, int C, double* dsums,
-                      const float* scale, const float* shift, void* stream);
-int pxl_bn_bwd_dx(const float* x, const float* y, const float* dy, const float* mean,
-                  const float* invstd, const float* gamma, const double* dsums, double count,
-                  int relu, float* dx, float* dres, int64_t rows, int C,
-                  const float* scale, const float* shift, float* dgamma_acc, float* dbeta_acc, void* stream);
-/* dgamma_acc / dbeta_acc (both or neither): dgamma_acc[c] += dsums[C+c], dbeta_acc[c] += dsums[c] by the same launch
- * (single-GPU path: dsums are the local sums; replaces pxl_bn_bwd_params + the optimizer-side accumulation). */
-/* fp16-pair variants (csrc/h16_prep.cu) of the BatchNorm launches: the SAME pass that writes y (dx) also, or only
- * (y / dx NULL), writes it as the fp16 pair the next wgmma convolution reads, so the pair costs no extra trip
- * through HBM.  hi / lo: __half NHWC planes, lo nullable.  Forward: fixed scale `hscale`.  Backward: the reduce
- * launch leaves absmax(dz) in slot[2] (DEVICE float[4], zeroed), the dx launch derives the power-of-two scale from
- * it, max|gamma*invstd| and target_log2, and stores s / 1/s in slot[0] / slot[1].
- * relu_mask (nullable, rows*C/4 bytes): the forward launches store the sign bits of the result (bit k of byte i =
- * element 4i+k > 0); the backward launches then take the ReLU mask from it instead of re-reading the fp32 result
- * (0.25 B/element instead of 4). */
-int pxl_bn_apply_h16(const float* x, const float* scale, const float* shift, const float* residual, int relu, float* y,
-                     int64_t rows, int C, void* hi, void* lo, float hscale, void* relu_mask, void* stream);
-int pxl_bn_finalize_apply_h16(const float* x, const double* sums, double count, const float* gamma, const float* beta,
-                              float* running_mean, float* running_var, float momentum, float eps, int clamp_mode,
-                              float* mean, float* invstd, float* scale, float* shift, const float* residual, int relu,
-                              float* y, int64_t rows, int C, void* hi, void* lo, float hscale, void* relu_mask,
-                              void* stream);
-int pxl_bn_bwd_reduce_h16(const float* x, const float* y, const float* dy, const float* mean, const float* invstd,
-                          int relu, int64_t rows, int C, double* dsums, const float* scale, const float* shift,
-                          float* amax_slot, const void* relu_mask, void* stream);
-int pxl_bn_bwd_dx_h16(const float* x, const float* y, const float* dy, const float* mean, const float* invstd,
-                      const float* gamma, const double* dsums, double count, int relu, float* dx, float* dres,
-                      int64_t rows, int C, const float* scale, const float* shift, float* dgamma_acc, float* dbeta_acc,
-                      void* dhi, void* dlo, float* slot, int target_log2, const void* relu_mask, void* stream);
+int pxl_bn_finalize_apply(const float* x, const double* sums, double count, const float* gamma, const float* beta,
+                          float* running_mean, float* running_var, float momentum, float eps, int clamp_mode,
+                          float* mean, float* invstd, float* scale, float* shift, const float* residual, int relu,
+                          float* y, int64_t rows, int C, void* hi, void* lo, float hscale, void* relu_mask,
+                          void* stream);
+int pxl_bn_bwd_reduce(const float* x, const float* y, const float* dy, const float* mean, const float* invstd,
+                      int relu, int64_t rows, int C, double* dsums, const float* scale, const float* shift,
+                      float* amax_slot, const void* relu_mask, void* stream);
+int pxl_bn_bwd_dx(const float* x, const float* y, const float* dy, const float* mean, const float* invstd,
+                  const float* gamma, const double* dsums, double count, int relu, float* dx, float* dres,
+                  int64_t rows, int C, const float* scale, const float* shift, float* dgamma_acc, float* dbeta_acc,
+                  void* dhi, void* dlo, float* slot, int target_log2, const void* relu_mask, void* stream);
 int pxl_bn_bwd_params(const double* dsums, int C, float* dgamma, float* dbeta, int accumulate,
                       void* stream);
 
@@ -259,11 +248,8 @@ int pxl_conv_wgrad_nhwc(const pxl_conv_geom* geom_host, const int* taps_dydx_hos
 /* wgmma path with explicit operands.  precision 1: in_lo / w_lo ignored (NULL).  precision 2
  * (3xTF32): in_hi/in_lo and w_hi/w_lo are the tf32 split of the fp32 tensors (pxl_split_tf32):
  * out = in_hi*w_hi + in_lo*w_hi + in_hi*w_lo accumulated in fp32 (registers).  Supports mul == div == 1
- * and Cin % 32 == 0; anything else returns PXL_ERR_UNSUPPORTED. */
-int pxl_conv_tc_launch(const pxl_conv_geom* geom_host, const int* taps_dydx_host, const float* in_hi,
-                       const float* in_lo, const float* w_hi, const float* w_lo, const float* bias,
-                       float* out, void* stream);
-/* Extended form used for strided convolutions:
+ * and Cin % 32 == 0; anything else returns PXL_ERR_UNSUPPORTED.  ext_host (nullable) extends this for strided
+ * convolutions:
  *  - geom.mul == 2 (stride-2 forward) is served by the TMA traversal stride;
  *  - stride-2 dgrad is decomposed by output parity into four stride-1 problems over dY: each launch
  *    passes the taps of one parity class (offsets already halved), `widx_host[t]` = index of tap t in
@@ -284,7 +270,7 @@ int pxl_conv_tc_launch_ex(const pxl_conv_geom* geom_host, const int* taps_dydx_h
                           const float* in_hi, const float* in_lo, const float* w_hi, const float* w_lo,
                           const float* bias, float* out, void* stream);
 /* wgmma wgrad (accumulates into dw): both operands MN-major via TMA, split over the pixel range,
- * fp32 RED epilogue.  Same precision / operand convention as pxl_conv_tc_launch; needs mul == div == 1,
+ * fp32 RED epilogue.  Same precision / operand convention as pxl_conv_tc_launch_ex; needs mul == div == 1,
  * Cin % 32 == 0 and ldo % 32 == 0. */
 int pxl_conv_wgrad_tc_launch(const pxl_conv_geom* geom_host, const int* taps_dydx_host, const float* in_hi,
                              const float* in_lo, const float* dy_hi, const float* dy_lo, float* dw,
@@ -309,7 +295,6 @@ int pxl_conv_wgrad_h16_launch(const pxl_conv_geom* geom_host, const int* taps_dy
 int pxl_h16_split(const float* x, void* hi, void* lo, int64_t n, float scale, float* slot, int target_log2,
                   void* stream);
 int pxl_h16_absmax(const float* x, int64_t n, float* slot, void* stream);
-int* pxl_h16_sat_counter(void);      /* DEVICE int[4] the producers of fp16 pairs add saturation events to */
 int pxl_h16_status(void);            /* number of threads that clipped a value since the last reset (synchronises) */
 int pxl_h16_status_sites(int* out4_host);   /* the same per producer: split fixed / split dynamic / BN apply / BN dx */
 int pxl_h16_reset_status(void);
@@ -432,12 +417,11 @@ int pxl_gaussian_noise(float* inp, const float* noise, int n, int64_t CHW, float
  * per-layer replica synchronisation (sync_batchnorm/batchnorm.py:55-78,90-125; comm.py) and, for the forward,
  * also _compute_mean_std: one single-CTA kernel pushes this rank's 2C fp64 sums into every rank's mailbox
  * (CUDA-IPC mapped), waits for all lanes, adds them in rank order and (count > 0) finalizes the layer.
- *   pxl_peer_alloc/export/open: mailbox of pxl_peer_mailbox_bytes() bytes, 64-byte IPC handle, peer mapping.
+ *   pxl_peer_alloc/export/open: mailbox (sized by the library), 64-byte IPC handle, peer mapping.
  *   pxl_peer_allreduce_bn: sums [n = 2C] in place; mailboxes = host array of `world` device pointers (own one at
  *   index rank); seq = 1, 2, 3, ... identical on all ranks; count <= 0: plain all-reduce (backward dsums), where
  *   dgamma_acc / dbeta_acc (both or neither) first receive += the LOCAL sums (the BN parameter gradients).
  * --------------------------------------------------------------------------------------------- */
-int64_t pxl_peer_mailbox_bytes(void);
 int pxl_peer_alloc(void** ptr);
 int pxl_peer_free(void* ptr);
 int pxl_peer_export(void* ptr, unsigned char* handle64);

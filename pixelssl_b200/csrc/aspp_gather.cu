@@ -78,8 +78,6 @@ aspp_scatter_h16_kernel(const float* __restrict__ dy, __half* __restrict__ hi, _
     if (clipped && sat) atomicAdd(sat, 1);
 }
 
-extern "C" int* pxl_h16_sat_counter(void);
-
 // dZ [N,H,W,ldz] as an fp16 pair (lo nullable): dZ[q, t*C + co] = dy[q - off_t, co] (zero outside the image and for
 // channels >= ntaps*C); scale from slot[2] = absmax(dy) bits (pxl_h16_absmax), s / 1/s stored in slot[0..1]
 extern "C" int pxl_aspp_scatter_h16(const float* dy, void* hi, void* lo, float* slot, int target_log2, int N, int H, int W,

@@ -7,6 +7,8 @@
 #define PXL_NUM_SMS 132
 
 extern "C" void pxl_count_launch_(int n);
+// DEVICE int[4] the producers of fp16 pairs add saturation events to (h16_prep.cu); nullptr if it could not be allocated
+extern "C" int* pxl_h16_sat_counter(void);
 
 // per-(purpose, stream) scratch buffer (conv_api.cu); *rc != 0 on failure
 #define PXL_WS_WGRAD 0

@@ -730,8 +730,6 @@ stem_im2col_h16_kernel(const float* __restrict__ img, uint2* __restrict__ hi, ui
     if (clipped && sat) atomicAdd(sat, 1);
 }
 
-extern "C" int* pxl_h16_sat_counter(void);
-
 // table: the geometry's constant-memory tap table, uploaded on the first call (the flag is per geometry)
 template <int KS, int PAD, int KH>
 static int stem_im2col_h16_run(const void* table, bool& uploaded, const float* img, void* hi, void* lo, float scale,

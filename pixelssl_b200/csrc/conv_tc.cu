@@ -670,16 +670,10 @@ static int conv_tc_launch_core(const pxl_conv_geom* g, const int* taps, const px
                                const float* bias, float* out, void* stream);
 
 // lo parts: for precision 2 the caller passes hi/lo through `in`/`w` (hi) and the extra pointers
-extern "C" int pxl_conv_tc_launch(const pxl_conv_geom* g, const int* taps, const float* in_hi, const float* in_lo,
-                                  const float* w_hi, const float* w_lo, const float* bias, float* out, void* stream) {
-    if (g && g->precision > 2) return PXL_ERR_BAD_ARG;      // fp16 operands go through pxl_conv_h16_launch
-    return conv_tc_launch_core(g, taps, nullptr, in_hi, in_lo, w_hi, w_lo, bias, out, stream);
-}
-
 extern "C" int pxl_conv_tc_launch_ex(const pxl_conv_geom* g, const int* taps, const pxl_conv_tc_ext* ext,
                                      const float* in_hi, const float* in_lo, const float* w_hi, const float* w_lo,
                                      const float* bias, float* out, void* stream) {
-    if (g && g->precision > 2) return PXL_ERR_BAD_ARG;
+    if (g && g->precision > 2) return PXL_ERR_BAD_ARG;      // fp16 operands go through pxl_conv_h16_launch
     return conv_tc_launch_core(g, taps, ext, in_hi, in_lo, w_hi, w_lo, bias, out, stream);
 }
 
@@ -793,8 +787,9 @@ extern "C" int pxl_conv_tc_status(void) {
 extern "C" int pxl_conv_tc_impl(const pxl_conv_geom* g, const int* taps, const float* in, const float* w,
                                 const float* bias, float* out, void* stream) {
     if (!g) return PXL_ERR_BAD_ARG;
-    if (g->precision == 2) return PXL_ERR_UNSUPPORTED;     // 3xTF32 needs the split operands: pxl_conv_tc_launch
-    return pxl_conv_tc_launch(g, taps, in, nullptr, w, nullptr, bias, out, stream);
+    if (g->precision == 2) return PXL_ERR_UNSUPPORTED;     // 3xTF32 needs the split operands: pxl_conv_tc_launch_ex
+    if (g->precision > 2) return PXL_ERR_BAD_ARG;          // fp16 operands go through pxl_conv_h16_launch
+    return conv_tc_launch_core(g, taps, nullptr, in, nullptr, w, nullptr, bias, out, stream);
 }
 
 // ==========================================================================================

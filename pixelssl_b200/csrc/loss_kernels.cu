@@ -16,7 +16,7 @@ extern "C" int pxl_pdl_enabled_(void) {
     if (v < 0) { const char* e = getenv("PXL_PDL"); v = e ? (atoi(e) != 0) : 1; }
     return v;
 }
-extern "C" int pxl_abi_version(void) { return 2; }   // 2: relu_mask argument of the pxl_bn_*_h16 entry points
+extern "C" int pxl_abi_version(void) { return 3; }   // 3: one BatchNorm entry point per launch (fp16-pair arguments included)
 extern "C" int64_t pxl_launch_count(void) { return g_launches; }
 extern "C" void pxl_reset_launch_count(void) { g_launches = 0; }
 

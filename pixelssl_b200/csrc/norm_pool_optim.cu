@@ -204,23 +204,11 @@ bn_apply_kernel(const float4* __restrict__ x, const float4* __restrict__ scale, 
     if (clipped && sat) atomicAdd(sat, 1);
 }
 
-extern "C" int* pxl_h16_sat_counter(void);
-
-extern "C" int pxl_bn_apply_h16(const float* x, const float* scale, const float* shift, const float* residual,
-                                int relu, float* y, int64_t rows, int C, void* hi, void* lo, float hscale, void* relu_mask,
-                                void* stream);
-
-extern "C" int pxl_bn_apply(const float* x, const float* scale, const float* shift, const float* residual,
-                            int relu, float* y, int64_t rows, int C, void* stream) {
-    if (!y) return PXL_ERR_BAD_ARG;
-    return pxl_bn_apply_h16(x, scale, shift, residual, relu, y, rows, C, nullptr, nullptr, 1.f, nullptr, stream);
-}
-
 // y nullable when the fp16 pair (hi, lo nullable) is the only output wanted; relu_mask (nullable, rows*C/4 bytes)
-// receives the sign bits of the result for the backward (pxl_bn_bwd_*_h16)
-extern "C" int pxl_bn_apply_h16(const float* x, const float* scale, const float* shift, const float* residual,
-                                int relu, float* y, int64_t rows, int C, void* hi, void* lo, float hscale, void* relu_mask,
-                                void* stream) {
+// receives the sign bits of the result for the backward (pxl_bn_bwd_*)
+extern "C" int pxl_bn_apply(const float* x, const float* scale, const float* shift, const float* residual,
+                            int relu, float* y, int64_t rows, int C, void* hi, void* lo, float hscale, void* relu_mask,
+                            void* stream) {
     if (!x || !scale || !shift || (!y && !hi) || rows <= 0 || C <= 0 || (C & 3)) return PXL_ERR_BAD_ARG;
     const int64_t n4 = rows * (C / 4);
     int blocks = (int)(pxl_cdiv(n4, 256 * 2) < PXL_NUM_SMS * 8 ? pxl_cdiv(n4, 256 * 2) : PXL_NUM_SMS * 8);
@@ -343,27 +331,12 @@ static RedLayout stream_layout(int64_t rows, int C) {
     return L;
 }
 
-extern "C" int pxl_bn_finalize_apply_h16(const float* x, const double* sums, double count, const float* gamma,
-                                         const float* beta, float* running_mean, float* running_var, float momentum,
-                                         float eps, int clamp_mode, float* mean, float* invstd, float* scale, float* shift,
-                                         const float* residual, int relu, float* y, int64_t rows, int C,
-                                         void* hi, void* lo, float hscale, void* relu_mask, void* stream);
-
+// the same launch also (or only: y nullable) writes the result as the fp16 pair the next convolution reads
 extern "C" int pxl_bn_finalize_apply(const float* x, const double* sums, double count, const float* gamma,
                                      const float* beta, float* running_mean, float* running_var, float momentum,
                                      float eps, int clamp_mode, float* mean, float* invstd, float* scale, float* shift,
-                                     const float* residual, int relu, float* y, int64_t rows, int C, void* stream) {
-    if (!y) return PXL_ERR_BAD_ARG;
-    return pxl_bn_finalize_apply_h16(x, sums, count, gamma, beta, running_mean, running_var, momentum, eps, clamp_mode, mean,
-                                     invstd, scale, shift, residual, relu, y, rows, C, nullptr, nullptr, 1.f, nullptr, stream);
-}
-
-// the same launch also (or only: y nullable) writes the result as the fp16 pair the next convolution reads
-extern "C" int pxl_bn_finalize_apply_h16(const float* x, const double* sums, double count, const float* gamma,
-                                         const float* beta, float* running_mean, float* running_var, float momentum,
-                                         float eps, int clamp_mode, float* mean, float* invstd, float* scale, float* shift,
-                                         const float* residual, int relu, float* y, int64_t rows, int C,
-                                         void* hi, void* lo, float hscale, void* relu_mask, void* stream) {
+                                     const float* residual, int relu, float* y, int64_t rows, int C,
+                                     void* hi, void* lo, float hscale, void* relu_mask, void* stream) {
     if (!x || !sums || !gamma || !beta || !mean || !invstd || !scale || !shift || (!y && !hi) || rows <= 0 || C <= 0 || (C & 3) || count <= 0)
         return PXL_ERR_BAD_ARG;
     int* sat = hi ? pxl_h16_sat_counter() : nullptr;
@@ -442,24 +415,13 @@ bn_bwd_reduce_kernel(const float* __restrict__ x, const float* __restrict__ y, c
     block_reduce_cols(s, q, TX, TY, c4, c4max, dsums, dsums + C);
 }
 
-extern "C" int pxl_bn_bwd_reduce_h16(const float* x, const float* y, const float* dy, const float* mean,
-                                     const float* invstd, int relu, int64_t rows, int C, double* dsums,
-                                     const float* scale, const float* shift, float* amax_slot, const void* relu_mask,
-                                     void* stream);
-
+// amax_slot (nullable DEVICE float[4], zeroed): slot[2] = max(slot[2], absmax(dz)) as a bit pattern
+// ReLU mask source, in this order: relu_mask (bytes written by pxl_bn_*apply), y (the forward result), else
+// recomputed from x*scale+shift (no residual)
 extern "C" int pxl_bn_bwd_reduce(const float* x, const float* y, const float* dy, const float* mean,
                                  const float* invstd, int relu, int64_t rows, int C, double* dsums,
-                                 const float* scale, const float* shift, void* stream) {
-    return pxl_bn_bwd_reduce_h16(x, y, dy, mean, invstd, relu, rows, C, dsums, scale, shift, nullptr, nullptr, stream);
-}
-
-// amax_slot (nullable DEVICE float[4], zeroed): slot[2] = max(slot[2], absmax(dz)) as a bit pattern
-// ReLU mask source, in this order: relu_mask (bytes written by pxl_bn_*apply_h16), y (the forward result), else
-// recomputed from x*scale+shift (no residual)
-extern "C" int pxl_bn_bwd_reduce_h16(const float* x, const float* y, const float* dy, const float* mean,
-                                     const float* invstd, int relu, int64_t rows, int C, double* dsums,
-                                     const float* scale, const float* shift, float* amax_slot, const void* relu_mask,
-                                     void* stream) {
+                                 const float* scale, const float* shift, float* amax_slot, const void* relu_mask,
+                                 void* stream) {
     if (!x || !dy || !mean || !invstd || !dsums || rows <= 0 || C <= 0 || (C & 3) || (relu && !y && !relu_mask && !(scale && shift))) return PXL_ERR_BAD_ARG;
     RedLayout L = red_layout(rows, C);
     dim3 grid(L.rowBlocks, L.colBlocks);
@@ -586,28 +548,13 @@ bn_bwd_dx_kernel(const float4* __restrict__ x, const float4* __restrict__ y, con
     if (clipped && sat) atomicAdd(sat, 1);
 }
 
-extern "C" int pxl_bn_bwd_dx_h16(const float* x, const float* y, const float* dy, const float* mean,
-                                 const float* invstd, const float* gamma, const double* dsums, double count,
-                                 int relu, float* dx, float* dres, int64_t rows, int C,
-                                 const float* scale, const float* shift, float* dgamma_acc, float* dbeta_acc,
-                                 void* dhi, void* dlo, float* slot, int target_log2, const void* relu_mask, void* stream);
-
+// dx also (or only: dx nullable) as the fp16 pair (dhi, dlo nullable) the dgrad / wgrad convolutions read; slot = the
+// DEVICE float[4] pxl_bn_bwd_reduce left absmax(dz) in: this launch stores the pair's scale s / 1/s in slot[0..1]
 extern "C" int pxl_bn_bwd_dx(const float* x, const float* y, const float* dy, const float* mean,
                              const float* invstd, const float* gamma, const double* dsums, double count,
                              int relu, float* dx, float* dres, int64_t rows, int C,
-                             const float* scale, const float* shift, float* dgamma_acc, float* dbeta_acc, void* stream) {
-    if (!dx) return PXL_ERR_BAD_ARG;
-    return pxl_bn_bwd_dx_h16(x, y, dy, mean, invstd, gamma, dsums, count, relu, dx, dres, rows, C, scale, shift,
-                             dgamma_acc, dbeta_acc, nullptr, nullptr, nullptr, 0, nullptr, stream);
-}
-
-// dx also (or only: dx nullable) as the fp16 pair (dhi, dlo nullable) the dgrad / wgrad convolutions read; slot = the
-// DEVICE float[4] pxl_bn_bwd_reduce_h16 left absmax(dz) in: this launch stores the pair's scale s / 1/s in slot[0..1]
-extern "C" int pxl_bn_bwd_dx_h16(const float* x, const float* y, const float* dy, const float* mean,
-                                 const float* invstd, const float* gamma, const double* dsums, double count,
-                                 int relu, float* dx, float* dres, int64_t rows, int C,
-                                 const float* scale, const float* shift, float* dgamma_acc, float* dbeta_acc,
-                                 void* dhi, void* dlo, float* slot, int target_log2, const void* relu_mask, void* stream) {
+                             const float* scale, const float* shift, float* dgamma_acc, float* dbeta_acc,
+                             void* dhi, void* dlo, float* slot, int target_log2, const void* relu_mask, void* stream) {
     if ((!dx && !dhi) || (dhi && !slot)) return PXL_ERR_BAD_ARG;
     int* sat = dhi ? pxl_h16_sat_counter() : nullptr;
     if (sat) sat += 3;

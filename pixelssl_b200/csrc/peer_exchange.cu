@@ -30,8 +30,6 @@ struct PxSlot {
 struct PxMailbox { PxSlot slot[PX_NSLOT]; };
 struct PxPeers { PxMailbox* box[PX_MAXW]; };
 
-extern "C" int64_t pxl_peer_mailbox_bytes(void) { return (int64_t)sizeof(PxMailbox); }
-
 extern "C" int pxl_peer_alloc(void** ptr) {
     if (!ptr) return PXL_ERR_BAD_ARG;
     cudaError_t e = cudaMalloc(ptr, sizeof(PxMailbox));

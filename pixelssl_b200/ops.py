@@ -1233,16 +1233,17 @@ def register_peer_exchange(group, exchange):
 
 
 def _bn_train_forward(x, sums, rows, C, gamma, beta, running_mean, running_var, momentum, eps, clamp_var, group, coeff,
-                      residual, relu, y, h16_out=()):
+                      residual, relu, y, h16_out=(None, None, 1.0, None)):
     """Train-mode (Sync)BN once its statistics ``sums`` exist: reduce them over ``group``, finalize (running statistics,
     mean / invstd / scale / shift into ``coeff``) and apply -> the element count the statistics cover.  Local: one
     finalize + apply launch.  Group: the peer exchange finalizes as it reduces (NCCL: all-reduce, then a finalize
-    launch), then an apply launch.  h16_out: the (hi, lo, scale, mask) arguments of the fp16-pair apply variants."""
+    launch), then an apply launch.  h16_out: the (hi, lo, scale, mask) arguments of the apply launch (default: no
+    fp16 pair, no mask)."""
     count, clamp = float(rows), 1 if clamp_var else 0
     if group is None:
-        call('pxl_bn_finalize_apply_h16' if h16_out else 'pxl_bn_finalize_apply', _p(x), _p(sums), count, _p(gamma),
-             _p(beta), _p(running_mean), _p(running_var), float(momentum), float(eps), clamp, _p(coeff[0]), _p(coeff[1]),
-             _p(coeff[2]), _p(coeff[3]), _p(residual), int(relu), _p(y), rows, C, *h16_out, _stream())
+        call('pxl_bn_finalize_apply', _p(x), _p(sums), count, _p(gamma), _p(beta), _p(running_mean), _p(running_var),
+             float(momentum), float(eps), clamp, _p(coeff[0]), _p(coeff[1]), _p(coeff[2]), _p(coeff[3]), _p(residual),
+             int(relu), _p(y), rows, C, *h16_out, _stream())
         return count
     import torch.distributed as dist
     count *= dist.get_world_size(group)
@@ -1256,8 +1257,8 @@ def _bn_train_forward(x, sums, rows, C, gamma, beta, running_mean, running_var, 
         dist.all_reduce(sums, group=group)
         call('pxl_bn_finalize', _p(sums), count, C, _p(gamma), _p(beta), _p(running_mean), _p(running_var),
              float(momentum), float(eps), clamp, _p(coeff[0]), _p(coeff[1]), _p(coeff[2]), _p(coeff[3]), _stream())
-    call('pxl_bn_apply_h16' if h16_out else 'pxl_bn_apply', _p(x), _p(coeff[2]), _p(coeff[3]), _p(residual), int(relu),
-         _p(y), rows, C, *h16_out, _stream())
+    call('pxl_bn_apply', _p(x), _p(coeff[2]), _p(coeff[3]), _p(residual), int(relu), _p(y), rows, C, *h16_out,
+         _stream())
     return count
 
 
@@ -1321,7 +1322,8 @@ class _BnAct(torch.autograd.Function):
                 # constants; mean / inv_std slots hold them for bn_bwd_reduce (tiny per-channel torch ops)
                 coeff[0].copy_(running_mean)
                 coeff[1].copy_(torch.rsqrt(running_var + eps))
-            call('pxl_bn_apply', _p(x), _p(coeff[2]), _p(coeff[3]), _p(residual), int(relu), _p(y), rows, C, _stream())
+            call('pxl_bn_apply', _p(x), _p(coeff[2]), _p(coeff[3]), _p(residual), int(relu), _p(y), rows, C,
+                 None, None, 1.0, None, _stream())
         ctx.save_for_backward(x, y if (relu and residual is not None) else None, gamma, coeff, running_var, beta)
         ctx.meta = (rows, C, count, bool(relu), residual is not None, bool(training), float(eps), group)
         return y
@@ -1336,7 +1338,7 @@ class _BnAct(torch.autograd.Function):
         # ReLU without residual: the mask is recomputed from x (same fmaf as the forward) instead of reading y
         ymask = y if (relu and has_res) else None
         call('pxl_bn_bwd_reduce', _p(x), _p(ymask), _p(dy), _p(coeff[0]), _p(coeff[1]), int(relu), rows, C, _p(dsums),
-             _p(coeff[2]), _p(coeff[3]), _stream())
+             _p(coeff[2]), _p(coeff[3]), None, None, _stream())
         if not training:
             # F.batch_norm(training=False) backward: dx = dz * gamma / sqrt(running_var + eps), d(gamma) = sum dz * xhat,
             # d(beta) = sum dz with xhat from the running statistics.  The reduce launch gives the parameter sums; the
@@ -1350,7 +1352,8 @@ class _BnAct(torch.autograd.Function):
         dx = torch.empty_like(x)
         dres = torch.empty_like(x) if has_res else None
         call('pxl_bn_bwd_dx', _p(x), _p(ymask), _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, int(relu),
-             _p(dx), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc), _stream())
+             _p(dx), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc), None, None, None, 0, None,
+             _stream())
         return dx, dgamma, dbeta, None, None, dres, None, None, None, None, None, None, None
 
 
@@ -1450,12 +1453,12 @@ class _ConvBnAct(torch.autograd.Function):
         slot = _scale_slot(dev)
         if relu and has_res and mask is None:
             raise RuntimeError('the ReLU mask of a residual unit was not recorded in the forward')
-        call('pxl_bn_bwd_reduce_h16', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), int(relu), rows, C, _p(dsums),
+        call('pxl_bn_bwd_reduce', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), int(relu), rows, C, _p(dsums),
              _p(coeff[2]), _p(coeff[3]), _p(slot), _p(mask), _stream())
         dgamma, dbeta, gacc, bacc = _bn_backward_sums(dsums, C, gamma, beta, group)
         dpair = torch.empty((2, n), dtype=torch.float16, device=dev)
         dres = torch.empty_like(c) if has_res else None
-        call('pxl_bn_bwd_dx_h16', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, int(relu),
+        call('pxl_bn_bwd_dx', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, int(relu),
              _p(None), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc),
              _p(dpair[0]), _p(dpair[1] if want_lo else None), _p(slot), H16_DX_TARGET_LOG2, _p(mask), _stream())
         dh = H16(dpair, n, None, slot, want_lo)
@@ -1623,11 +1626,11 @@ class _DwBnPair(torch.autograd.Function):
         rows, dev = N * OH * OW, dy.device
         dsums = _stat_zeros(2 * ld, dev)
         call('pxl_bn_bwd_reduce', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), 0, rows, ld, _p(dsums),
-             _p(coeff[2]), _p(coeff[3]), _stream())
+             _p(coeff[2]), _p(coeff[3]), None, None, _stream())
         dgamma, dbeta, gacc, bacc = _bn_backward_sums(dsums, ld, gamma, beta, group)
         dc = torch.empty_like(c)
         call('pxl_bn_bwd_dx', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, 0,
-             _p(dc), None, rows, ld, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc), _stream())
+             _p(dc), None, rows, ld, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc), None, None, None, 0, None, _stream())
         dx, dw = _dw_backward(x, weight, dc, ctx.meta, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
         return (dx, dw, dgamma, dbeta) + (None,) * 8
 
@@ -1959,7 +1962,8 @@ class _IBNorm(torch.autograd.Function):
         for i in range(b):
             call('pxl_bn_finalize', _p(mix[i]), float(hw), C, _p(gamma), _p(beta), _p(None), _p(None), 0.0, float(eps), 0,
                  _p(coeff[i, 0]), _p(coeff[i, 1]), _p(coeff[i, 2]), _p(coeff[i, 3]), _stream())
-            call('pxl_bn_apply', _p(x[i]), _p(coeff[i, 2]), _p(coeff[i, 3]), _p(None), 0, _p(y[i]), hw, C, _stream())
+            call('pxl_bn_apply', _p(x[i]), _p(coeff[i, 2]), _p(coeff[i, 3]), _p(None), 0, _p(y[i]), hw, C,
+                 None, None, 1.0, None, _stream())
         # running statistics of the BN half (unbiased variance over all rows)
         bn_sums = torch.cat((sums_all[:nb], sums_all[C:C + nb])).contiguous()
         scratch = torch.empty((4, nb), dtype=torch.float32, device=dev)
@@ -1978,7 +1982,7 @@ class _IBNorm(torch.autograd.Function):
         dsums = torch.zeros((b, 2 * C), dtype=torch.float64, device=dev)
         for i in range(b):
             call('pxl_bn_bwd_reduce', _p(x[i]), _p(None), _p(dy[i]), _p(coeff[i, 0]), _p(coeff[i, 1]), 0, hw, C,
-                 _p(dsums[i]), _p(None), _p(None), _stream())
+                 _p(dsums[i]), _p(None), _p(None), None, None, _stream())
         tot = dsums.sum(0)
         dgamma = tot[C:C + nb].to(torch.float32)
         dbeta = tot[:nb].to(torch.float32)
@@ -1992,7 +1996,8 @@ class _IBNorm(torch.autograd.Function):
         dx = torch.empty_like(x)
         for i in range(b):
             call('pxl_bn_bwd_dx', _p(x[i]), _p(None), _p(dy[i]), _p(coeff[i, 0]), _p(coeff[i, 1]), _p(gamma), _p(mix[i]),
-                 float(hw), 0, _p(dx[i]), _p(None), hw, C, _p(None), _p(None), _p(None), _p(None), _stream())
+                 float(hw), 0, _p(dx[i]), _p(None), hw, C, _p(None), _p(None), _p(None), _p(None),
+                 None, None, None, 0, None, _stream())
         return dx, dgamma, dbeta, None, None, None, None, None, None
 
 

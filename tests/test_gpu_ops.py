@@ -237,7 +237,7 @@ def test_bn_act_train(ops, N, C, H, W, relu, res):
         assert rel(rg.grad, rc.grad) <= 1e-6
 
 @pytest.mark.parametrize('rows,C', [(1000, 64), (33 * 33 * 2, 256), (77, 2048)])
-def test_bn_backward_relu_byte_mask_equals_the_fp32_result_mask(ops, rows, C):
+def test_bn_relu_byte_mask_equals_the_fp32_result_mask(ops, rows, C):
     """Block outputs record sign bits (1 byte per 4 values) in the forward apply; the backward launches that read
     them must produce bit-identical sums, dX pair and residual gradient to the launches that re-read the fp32 result."""
     from pixelssl_b200._lib import call
@@ -256,7 +256,7 @@ def test_bn_backward_relu_byte_mask_equals_the_fp32_result_mask(ops, rows, C):
     pair = torch.empty(2, rows * C, dtype=torch.float16, device=dev)
     mask = torch.zeros(rows * C // 4, dtype=torch.uint8, device=dev)
     st = ops._stream()
-    call('pxl_bn_finalize_apply_h16', P(x), P(sums), float(rows), P(gamma), P(beta), P(rm), P(rv), 0.1, 1e-5, 0,
+    call('pxl_bn_finalize_apply', P(x), P(sums), float(rows), P(gamma), P(beta), P(rm), P(rv), 0.1, 1e-5, 0,
          P(coeff[0]), P(coeff[1]), P(coeff[2]), P(coeff[3]), P(res), 1, P(y), rows, C, P(pair[0]), P(pair[1]), 16.0, P(mask), st)
     bits = (y.view(-1, 4) > 0).to(torch.uint8)
     want = bits[:, 0] | (bits[:, 1] << 1) | (bits[:, 2] << 2) | (bits[:, 3] << 3)
@@ -266,7 +266,7 @@ def test_bn_backward_relu_byte_mask_equals_the_fp32_result_mask(ops, rows, C):
     for use_mask in (False, True):
         dsums = torch.zeros(2 * C, dtype=torch.float64, device=dev)
         slot = torch.zeros(4, device=dev)
-        call('pxl_bn_bwd_reduce_h16', P(x), P(None if use_mask else y), P(dy), P(coeff[0]), P(coeff[1]), 1, rows, C, P(dsums),
+        call('pxl_bn_bwd_reduce', P(x), P(None if use_mask else y), P(dy), P(coeff[0]), P(coeff[1]), 1, rows, C, P(dsums),
              P(coeff[2]), P(coeff[3]), P(slot), P(mask if use_mask else None), st)
         if ds_ref is None:
             ds_ref = dsums.clone()
@@ -276,7 +276,7 @@ def test_bn_backward_relu_byte_mask_equals_the_fp32_result_mask(ops, rows, C):
         dpair = torch.empty(2, rows * C, dtype=torch.float16, device=dev)
         dres = torch.empty_like(x)
         dx = torch.empty_like(x)
-        call('pxl_bn_bwd_dx_h16', P(x), P(None if use_mask else y), P(dy), P(coeff[0]), P(coeff[1]), P(gamma), P(ds_ref), float(rows), 1,
+        call('pxl_bn_bwd_dx', P(x), P(None if use_mask else y), P(dy), P(coeff[0]), P(coeff[1]), P(gamma), P(ds_ref), float(rows), 1,
              P(dx), P(dres), rows, C, P(coeff[2]), P(coeff[3]), P(None), P(None), P(dpair[0]), P(dpair[1]), P(slot), 12,
              P(mask if use_mask else None), st)
         torch.cuda.synchronize()

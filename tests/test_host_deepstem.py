@@ -216,13 +216,3 @@ def test_auto_is_refused(refuse, backbone):
     assert eng_model.pretrained_backbone_url(types.SimpleNamespace(backbone=backbone, pretrained_backbone='none')) is None
     assert eng_model.pretrained_backbone_url(types.SimpleNamespace(backbone='resnet101', pretrained_backbone='auto')) == \
         eng_model.PRETRAINED_BACKBONE_URLS['resnet101']
-
-
-def test_new_entry_points_are_declared():
-    import os
-    import re
-    from pixelssl_b200 import _lib
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    header = open(os.path.join(root, 'include', 'pixelssl_b200.h')).read()
-    for name in ('pxl_stem3x3s2_im2col', 'pxl_stem3x3s2_im2col_h16'):
-        assert re.search(r'\b%s\s*\(' % name, header) and name in _lib.SIGNATURES

@@ -266,13 +266,3 @@ def test_oracle_equals_module_restatement(output_stride, training):
         for k, v in ref.state_dict().items():
             if k.endswith('running_mean') or k.endswith('running_var'):
                 assert float((st['backbone.' + k] - v).abs().max()) < 1e-12, k
-
-
-def test_new_entry_points_are_declared():
-    import os
-    import re
-    from pixelssl_b200 import _lib
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    header = open(os.path.join(root, 'include', 'pixelssl_b200.h')).read()
-    for name in ('pxl_dw_conv_fwd', 'pxl_dw_conv_dgrad', 'pxl_dw_conv_wgrad'):
-        assert re.search(r'\b%s\s*\(' % name, header) and name in _lib.SIGNATURES

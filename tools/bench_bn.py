@@ -32,15 +32,16 @@ for name, rows, C in SHAPES:
     coeff = torch.rand(4, C, device='cuda') + 0.5
     gamma = torch.rand(C, device='cuda')
     sums = torch.zeros(2 * C, dtype=torch.float64, device='cuda')
-    t_apply = timeit(lambda: call('pxl_bn_apply', P(x), P(coeff[2]), P(coeff[3]), P(res), 1, P(y), rows, C, st))
-    t_red = timeit(lambda: call('pxl_bn_bwd_reduce', P(x), P(y), P(dy), P(coeff[0]), P(coeff[1]), 1, rows, C, P(sums), P(None), P(None), st))
+    t_apply = timeit(lambda: call('pxl_bn_apply', P(x), P(coeff[2]), P(coeff[3]), P(res), 1, P(y), rows, C, P(None), P(None), 1.0, P(None), st))
+    t_red = timeit(lambda: call('pxl_bn_bwd_reduce', P(x), P(y), P(dy), P(coeff[0]), P(coeff[1]), 1, rows, C, P(sums), P(None), P(None), P(None), P(None), st))
     t_dx = timeit(lambda: call('pxl_bn_bwd_dx', P(x), P(y), P(dy), P(coeff[0]), P(coeff[1]), P(gamma), P(sums), float(rows), 1,
-                               P(dx), P(dres), rows, C, P(None), P(None), P(None), P(None), st))
+                               P(dx), P(dres), rows, C, P(None), P(None), P(None), P(None), P(None), P(None), P(None), 0, P(None), st))
     rm, rv = torch.zeros(C, device='cuda'), torch.ones(C, device='cuda')
     beta = torch.rand(C, device='cuda')
     sums2 = torch.cat((x.double().sum(0), (x.double() ** 2).sum(0)))
     t_fa = timeit(lambda: call('pxl_bn_finalize_apply', P(x), P(sums2), float(rows), P(gamma), P(beta), P(rm), P(rv), 0.1, 1e-5, 0,
-                               P(coeff[0]), P(coeff[1]), P(coeff[2]), P(coeff[3]), P(res), 1, P(y), rows, C, st))
+                               P(coeff[0]), P(coeff[1]), P(coeff[2]), P(coeff[3]), P(res), 1, P(y), rows, C, P(None), P(None), 1.0,
+                               P(None), st))
     t_st = timeit(lambda: call('pxl_bn_stats', P(x), rows, C, P(sums), st))
     print('%-18s %6.1f MB  apply(+res,relu) %6.1f us %5.0f GB/s | fused fin+apply %6.1f us | bwd_reduce %6.1f us %5.0f GB/s | bwd_dx(+dres) %6.1f us %5.0f GB/s | stats %6.1f us %5.0f GB/s'
           % (name, n * 4 / 1e6, t_apply, 16 * n / t_apply / 1e3, t_fa, t_red, 12 * n / t_red / 1e3, t_dx, 20 * n / t_dx / 1e3, t_st, 4 * n / t_st / 1e3))

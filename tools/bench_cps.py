@@ -62,7 +62,7 @@ def engine(args, batches):
     torch.cuda.empty_cache()
     return {'value': (args.lbs + args.ubs) * args.steps / (ms / 1e3), 'unit': 'images/s', 'ms_per_step': ms / args.steps,
             'peak_mem_gib': peak / 2 ** 30, 'losses': losses, 'conv_precision': args.precision,
-            'pxl_cps_ce_one_step': launches, 'status': status}
+            'cps_ce_launches_one_step': launches, 'status': status}
 
 
 def stock_torch(args, batches):

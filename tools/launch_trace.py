@@ -5,8 +5,8 @@ in the same order with the same arguments print the same text.
 
 CONFIGS: comma list of bench.CONFIGS names, or 'mt_v3plus' (Mean-Teacher with the DeepLabV3+ task model); PRECISIONS:
 comma list of ops.PRECISION names.  Per pair: WARMUP (default 2) untraced steps, then one traced step.  Pointer arguments
-print as null / ptr (addresses differ between runs), scalars by value, ConvGeom / ConvTcExt fields and the tap /
-weight-index arrays expanded."""
+print as null / ptr (addresses differ between runs), scalars by value, ConvGeom / ConvTcExt fields expanded, host arrays
+of pointers as lists of null / ptr and other host arrays (taps, weight indices) by value."""
 import ctypes
 import logging
 import os
@@ -44,10 +44,10 @@ def fmt(name, args):
                     v = list(v[:ntaps]) if v else 'null'
                 fields.append('%s=%s' % (f, v))
             parts.append('{%s}' % ' '.join(fields))
-        elif t is ctypes.c_void_p or t is ctypes.POINTER(ctypes.c_void_p) or isinstance(a, ctypes.c_void_p):
-            parts.append(str(_ptr(a)))
         elif isinstance(a, ctypes.Array):
-            parts.append(str(list(a)))
+            parts.append(str(_ptr(a) if a._type_ is ctypes.c_void_p else list(a)))
+        elif t is ctypes.c_void_p:
+            parts.append(_ptr(a))
         else:
             parts.append(repr(a))
     return '%s(%s)' % (name, ', '.join(parts))
