@@ -9,9 +9,6 @@ Device-side replacements of the reference's host round trips: ``ssladv_preproces
 ``FCDiscriminatorCriterion`` (numpy masks every step, task/sseg/func.py:137-155) are one masked-BCE
 kernel; ``ssladv_convert_task_gt_to_fcd_input`` (numpy one-hot, func.py:157-168) is one kernel that
 writes the NHWC one-hot the first discriminator convolution reads."""
-import os
-import time
-
 import torch
 import torch.nn as nn
 import torch.optim as optim
@@ -75,6 +72,14 @@ class FCDiscriminator(nn.Module):
 class SSLADV(ssl_base._SSLBase):
     NAME = 'ssl_adv'
     SUPPORTED_TASK_TYPES = [REGRESSION, CLASSIFICATION]
+    LOG_LINES = ('  task-{3}\t=>\t'
+                 'task-loss: {meters[task_loss]:.6f}\t'
+                 'labeled-adv-loss: {meters[labeled_adv_loss]:.6f}\t'
+                 'unlabeled-adv-loss: {meters[unlabeled_adv_loss]:.6f}\n'
+                 '  fc-discriminator\t=>\t'
+                 'fake-d-loss: {meters[fake_d_loss]:.6f}\t'
+                 'real-d-loss: {meters[real_d_loss]:.6f}\n')
+    ITER_LRERS = ('d_lrer',)
 
     def __init__(self, args):
         super().__init__(args)
@@ -101,7 +106,7 @@ class SSLADV(ssl_base._SSLBase):
         self.criterion = criterion_funcs[0](self.args)
         self.criterions = {'criterion': self.criterion, 'd_criterion': ops.bce_logits_masked}
 
-    def train_step(self, inp, gt):
+    def train_step(self, inp, gt, cur_step, total_steps):
         lbs, bs = self.args.labeled_batch_size, self.args.batch_size
         ignore = self.args.ignore_index
         inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
@@ -159,61 +164,6 @@ class SSLADV(ssl_base._SSLBase):
         d_arena.all_reduce_grads()
         d_arena.adam_step(self.d_optimizer)
 
-    def _train(self, data_loader, epoch):
-        self.meters.reset()
-        self.model.train()
-        self.d_model.train()
-        for idx, (inp, gt) in enumerate(ssl_base.device_prefetch(data_loader)):
-            timer = time.time()
-            self.train_step(inp, gt)
-            self.meters.update('batch_time', time.time() - timer)
-            if idx % self.args.log_freq == 0:
-                self._log_step(lambda m, a=(epoch + 1, idx, len(data_loader), self.args.task): ('step: [{0}][{1}/{2}]\tbatch-time: {meters[batch_time]:.3f}\n'
-                                '  task-{3}\t=>\t'
-                                'task-loss: {meters[task_loss]:.6f}\t'
-                                'labeled-adv-loss: {meters[labeled_adv_loss]:.6f}\t'
-                                'unlabeled-adv-loss: {meters[unlabeled_adv_loss]:.6f}\n'
-                                '  fc-discriminator\t=>\t'
-                                'fake-d-loss: {meters[fake_d_loss]:.6f}\t'
-                                'real-d-loss: {meters[real_d_loss]:.6f}\n'
-                                ).format(*a, meters=m))
-            self.d_lrer.step()
-            if not self.args.is_epoch_lrer:
-                self.lrer.step()
-        if self.args.is_epoch_lrer:
-            self.lrer.step()
-
-    def _validate(self, data_loader, epoch):
-        self.meters.reset()
-        self.model.eval()
-        self.d_model.eval()
-        for idx, (inp, gt) in enumerate(data_loader):
-            inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
-            resulter, _ = self.model.forward(inp)
-            pred = tool.dict_value(resulter, 'pred')
-            self.meters.update('task_loss', torch.mean(self.criterion.forward(pred, gt, inp)).data)
-            self._metrics(resulter, gt, inp, 'task')
-        self._log_validation_metrics(('task',))
-
-    def _save_checkpoint(self, epoch):
-        state = {'algorithm': self.NAME, 'epoch': epoch,
-                 'model': self.model.state_dict(), 'd_model': self.d_model.state_dict(),
-                 'optimizer': self.optimizer.state_dict(), 'd_optimizer': self.d_optimizer.state_dict(),
-                 'lrer': self.lrer.state_dict(), 'd_lrer': self.d_lrer.state_dict()}
-        torch.save(state, os.path.join(self.args.checkpoint_path, 'checkpoint_{0}.ckpt'.format(epoch)))
-
-    def _load_checkpoint(self):
-        checkpoint = torch.load(self.args.resume, weights_only=False)
-        name = tool.dict_value(checkpoint, 'algorithm', default='unknown')
-        if name != self.NAME:
-            logger.log_err('Unmatched SSL algorithm format in checkpoint => required: {0} - given: {1}\n'
-                           .format(self.NAME, name))
-        self.model.load_state_dict(checkpoint['model'])
-        self.d_model.load_state_dict(checkpoint['d_model'])
-        self.optimizer.load_state_dict(checkpoint['optimizer'])
-        self.model.arena.adopt_optimizer_state(self.optimizer)
-        self.d_optimizer.load_state_dict(checkpoint['d_optimizer'])
-        self.d_model.arena.adopt_optimizer_state(self.d_optimizer)      # Adam moments + step count
-        self.lrer.load_state_dict(checkpoint['lrer'])
-        self.d_lrer.load_state_dict(checkpoint['d_lrer'])
-        return checkpoint['epoch']
+    def validate_step(self, inp, gt):
+        inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
+        self._validate_model(self.model, self.criterion, inp, gt, 'task_loss', 'task')

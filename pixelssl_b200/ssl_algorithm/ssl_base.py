@@ -3,7 +3,12 @@
 ``build / train / validate / save_checkpoint / load_checkpoint`` plus ``NAME`` and
 ``SUPPORTED_TASK_TYPES``.  TaskProxy (task_template/proxy.py:134-159,433-441) only ever touches
 these."""
-from ..utils import logger
+import os
+import time
+
+import torch
+
+from ..utils import logger, tool
 from ..task.sseg import evaluation
 
 
@@ -14,6 +19,10 @@ def add_parser_arguments(parser):
 class _SSLBase:
     NAME = 'ssl_base'
     SUPPORTED_TASK_TYPES = []
+    RAMPUP_EPOCHS = None         # name of the ramp-up argument (e.g. 'cons_rampup_epochs'); None: total_steps = 0
+    LOG_LINES = ''               # the step log line after the shared 'step: ... batch-time: ...' line
+    ITER_LRERS = ()              # keys of self.lrers stepped every iteration whatever is_epoch_lrer says
+    VALIDATION_IDS = ('task',)   # the id_str of every _metrics call of validate_step
 
     def __init__(self, args):
         self.args = args
@@ -54,10 +63,72 @@ class _SSLBase:
             logger.log_info(prev[0](prev[1]))
 
     def save_checkpoint(self, epoch):
-        self._save_checkpoint(epoch)
+        """``{'algorithm', 'epoch'}`` plus the state dict of every model, optimizer and lr scheduler under its key
+        in ``self.models`` / ``self.optimizers`` / ``self.lrers``: the reference's checkpoint layout
+        (e.g. ssl_mt.py:296-307)."""
+        state = {'algorithm': self.NAME, 'epoch': epoch}
+        for elements in (self.models, self.optimizers, self.lrers):
+            state.update((key, element.state_dict()) for key, element in elements.items())
+        torch.save(state, os.path.join(self.args.checkpoint_path, 'checkpoint_{0}.ckpt'.format(epoch)))
 
     def load_checkpoint(self):
-        return self._load_checkpoint()
+        """Loads ``args.resume`` into every model, optimizer and lr scheduler; the loaded momentum buffers / Adam
+        moments of optimizer ``x_optimizer`` move into the parameter arena of model ``x_model``.  Returns the
+        epoch."""
+        checkpoint = torch.load(self.args.resume, weights_only=False)
+        name = tool.dict_value(checkpoint, 'algorithm', default='unknown')
+        if name != self.NAME:
+            logger.log_err('Unmatched SSL algorithm format in checkpoint => required: {0} - given: {1}\n'
+                           .format(self.NAME, name))
+        for key, model in self.models.items():
+            model.load_state_dict(checkpoint[key])
+        for key, optimizer in self.optimizers.items():
+            optimizer.load_state_dict(checkpoint[key])
+            self.models[key.replace('optimizer', 'model')].arena.adopt_optimizer_state(optimizer)
+        for key, lrer in self.lrers.items():
+            lrer.load_state_dict(checkpoint[key])
+        return checkpoint['epoch']
+
+    def _train(self, data_loader, epoch):
+        """One epoch of every reference ``_train`` (e.g. ssl_mt.py:124-224): ``train_step`` per batch, timed, a step
+        log line every ``log_freq`` steps and the lr schedulers stepped per iteration or per epoch."""
+        self.meters.reset()
+        for model in self.models.values():
+            model.train()
+        rampup_epochs = getattr(self.args, self.RAMPUP_EPOCHS) if self.RAMPUP_EPOCHS else 0
+        line = 'step: [{0}][{1}/{2}]\tbatch-time: {meters[batch_time]:.3f}\n' + self.LOG_LINES
+        for idx, (inp, gt) in enumerate(device_prefetch(data_loader)):
+            timer = time.time()
+            cur_step = len(data_loader) * epoch + idx
+            total_steps = len(data_loader) * rampup_epochs
+            self.train_step(inp, gt, cur_step, total_steps)
+            self.meters.update('batch_time', time.time() - timer)
+            if idx % self.args.log_freq == 0:
+                self._log_step(lambda m, a=(epoch + 1, idx, len(data_loader), self.args.task): line.format(*a, meters=m))
+            for key, lrer in self.lrers.items():
+                if key in self.ITER_LRERS or not self.args.is_epoch_lrer:
+                    lrer.step()
+        if self.args.is_epoch_lrer:
+            for key, lrer in self.lrers.items():
+                if key not in self.ITER_LRERS:
+                    lrer.step()
+
+    def _validate(self, data_loader, epoch):
+        """Every reference ``_validate`` (e.g. ssl_mt.py:226-294): eval mode, ``validate_step`` per batch, then the
+        'Validation metrics' summary."""
+        self.meters.reset()
+        for model in self.models.values():
+            model.eval()
+        for inp, gt in data_loader:
+            self.validate_step(inp, gt)
+        self._log_validation_metrics(self.VALIDATION_IDS)
+
+    def _validate_model(self, model, criterion, inp, gt, meter, id_str):
+        """The validation body of one task model: forward, mean task loss into ``meter``, metrics under ``id_str``."""
+        resulter, _ = model.forward(inp)
+        pred = tool.dict_value(resulter, 'pred')
+        self.meters.update(meter, torch.mean(criterion.forward(pred, gt, inp)).data)
+        self._metrics(resulter, gt, inp, id_str)
 
     def _metrics(self, resulter, gt, inp, id_str):
         """``self.task_func.metrics(activated_pred, gt, inp, self.meters, id_str=...)`` of every
@@ -83,23 +154,17 @@ class _SSLBase:
             '  {0}-metrics\t=>\t{1}\n'.format(i, info[i].replace('_', '-')) for i in id_strs))
 
     def _pred_err(self):
-        logger.log_err('In SSL_{0}, the \'resulter\' dict returned by the task model should contain the following keys:\n'
+        logger.log_err('In {0}, the \'resulter\' dict returned by the task model should contain the following keys:\n'
                        '   (1) \'pred\'\t=>\tunactivated task predictions\n'
                        '   (2) \'activated_pred\'\t=>\tactivated task predictions\n'.format(self.NAME.upper()))
 
     def _build(self, model_funcs, optimizer_funcs, lrer_funcs, criterion_funcs, task_func):
         raise NotImplementedError
 
-    def _train(self, data_loader, epoch):
+    def train_step(self, inp, gt, cur_step, total_steps):
         raise NotImplementedError
 
-    def _validate(self, data_loader, epoch):
-        raise NotImplementedError
-
-    def _save_checkpoint(self, epoch):
-        raise NotImplementedError
-
-    def _load_checkpoint(self):
+    def validate_step(self, inp, gt):
         raise NotImplementedError
 
 
@@ -115,7 +180,6 @@ def device_prefetch(data_loader):
     The device side is two fixed staging slots (allocated once per tensor shape): slot k % 2 is rewritten only after
     the step that consumed it has finished, so no allocator traffic (and no cudaMalloc stall) sits in the loop.  A
     yielded batch is valid until the iteration after next."""
-    import torch
     if not torch.cuda.is_available():
         for batch in data_loader:
             yield batch

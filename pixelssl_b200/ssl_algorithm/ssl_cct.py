@@ -12,9 +12,7 @@ Random draws use the same host generators in the same order as the reference (py
 seeded run reproduces the reference's perturbations; Dropout2d's per-(sample, channel) mask is
 drawn with the CPU generator as well."""
 import math
-import os
 import random
-import time
 
 import numpy as np
 import torch
@@ -248,6 +246,8 @@ class WrappedCCTModel(nn.Module):
 class SSLCCT(ssl_base._SSLBase):
     NAME = 'ssl_cct'
     SUPPORTED_TASK_TYPES = [CLASSIFICATION]
+    RAMPUP_EPOCHS = 'cons_rampup_epochs'
+    LOG_LINES = '  task-{3}\t=>\ttask-loss: {meters[task_loss]:.6f}\tcons-loss: {meters[cons_loss]:.6f}\n'
 
     def __init__(self, args):
         super().__init__(args)
@@ -310,47 +310,8 @@ class SSLCCT(ssl_base._SSLBase):
         arena.all_reduce_grads()
         arena.sgd_step(self.optimizer)
 
-    def _train(self, data_loader, epoch):
-        self.meters.reset()
-        self.model.train()
-        for idx, (inp, gt) in enumerate(ssl_base.device_prefetch(data_loader)):
-            timer = time.time()
-            cur_step = len(data_loader) * epoch + idx
-            total_steps = len(data_loader) * self.args.cons_rampup_epochs
-            self.train_step(inp, gt, cur_step, total_steps)
-            self.meters.update('batch_time', time.time() - timer)
-            if idx % self.args.log_freq == 0:
-                self._log_step(lambda m, a=(epoch + 1, idx, len(data_loader), self.args.task): ('step: [{0}][{1}/{2}]\tbatch-time: {meters[batch_time]:.3f}\n'
-                                '  task-{3}\t=>\ttask-loss: {meters[task_loss]:.6f}\tcons-loss: {meters[cons_loss]:.6f}\n'
-                                ).format(*a, meters=m))
-            if not self.args.is_epoch_lrer:
-                self.lrer.step()
-        if self.args.is_epoch_lrer:
-            self.lrer.step()
-
-    def _validate(self, data_loader, epoch):
-        self.meters.reset()
-        self.model.eval()
-        for idx, (inp, gt) in enumerate(data_loader):
-            inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
-            resulter, _ = self.model.forward(inp, gt, False)
-            self.meters.update('task_loss', tool.dict_value(resulter, 'task_loss', err=True).mean().data)
-            self._metrics(resulter, gt, inp, 'task')
-        self._log_validation_metrics(('task',))
-
-    def _save_checkpoint(self, epoch):
-        state = {'algorithm': self.NAME, 'epoch': epoch, 'model': self.model.state_dict(),
-                 'optimizer': self.optimizer.state_dict(), 'lrer': self.lrer.state_dict()}
-        torch.save(state, os.path.join(self.args.checkpoint_path, 'checkpoint_{0}.ckpt'.format(epoch)))
-
-    def _load_checkpoint(self):
-        checkpoint = torch.load(self.args.resume, weights_only=False)
-        name = tool.dict_value(checkpoint, 'algorithm', default='unknown')
-        if name != self.NAME:
-            logger.log_err('Unmatched SSL algorithm format in checkpoint => required: {0} - given: {1}\n'
-                           .format(self.NAME, name))
-        self.model.load_state_dict(checkpoint['model'])
-        self.optimizer.load_state_dict(checkpoint['optimizer'])
-        self.model.arena.adopt_optimizer_state(self.optimizer)
-        self.lrer.load_state_dict(checkpoint['lrer'])
-        return checkpoint['epoch']
+    def validate_step(self, inp, gt):
+        inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
+        resulter, _ = self.model.forward(inp, gt, False)
+        self.meters.update('task_loss', tool.dict_value(resulter, 'task_loss', err=True).mean().data)
+        self._metrics(resulter, gt, inp, 'task')

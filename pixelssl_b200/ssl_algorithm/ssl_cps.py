@@ -10,9 +10,6 @@ the sum, SGD on each model.
 CutMix step (``--cps-cutmix``, the paper's VOC configuration): per model a forward of the labeled rows + task
 criterion, a no-grad forward of the unlabeled rows whose two halves are mixed with the box mask (the pseudo-label
 source), and a forward of the mixed images, which the CPS term supervises."""
-import os
-import time
-
 import torch
 
 from .. import ops
@@ -40,6 +37,10 @@ def ssl_cps(args, model_dict, optimizer_dict, lrer_dict, criterion_dict, task_fu
 class SSLCPS(ssl_base._SSLBase):
     NAME = 'ssl_cps'
     SUPPORTED_TASK_TYPES = [CLASSIFICATION]
+    RAMPUP_EPOCHS = 'cps_rampup_epochs'
+    LOG_LINES = ('  l-{3}\t=>\tl-task-loss: {meters[l_task_loss]:.6f}\tl-cps-loss: {meters[l_cps_loss]:.6f}\n'
+                 '  r-{3}\t=>\tr-task-loss: {meters[r_task_loss]:.6f}\tr-cps-loss: {meters[r_cps_loss]:.6f}\n')
+    VALIDATION_IDS = ('l', 'r')
 
     def __init__(self, args):
         super().__init__(args)
@@ -145,54 +146,7 @@ class SSLCPS(ssl_base._SSLBase):
             model.arena.all_reduce_grads()
             model.arena.sgd_step(opt)
 
-    def _train(self, data_loader, epoch):
-        self.meters.reset()
-        self.l_model.train(); self.r_model.train()
-        for idx, (inp, gt) in enumerate(ssl_base.device_prefetch(data_loader)):
-            timer = time.time()
-            cur_step = len(data_loader) * epoch + idx
-            total_steps = len(data_loader) * self.args.cps_rampup_epochs
-            self.train_step(inp, gt, cur_step, total_steps)
-            self.meters.update('batch_time', time.time() - timer)
-            if idx % self.args.log_freq == 0:
-                self._log_step(lambda m, a=(epoch + 1, idx, len(data_loader), self.args.task): ('step: [{0}][{1}/{2}]\tbatch-time: {meters[batch_time]:.3f}\n'
-                                '  l-{3}\t=>\tl-task-loss: {meters[l_task_loss]:.6f}\tl-cps-loss: {meters[l_cps_loss]:.6f}\n'
-                                '  r-{3}\t=>\tr-task-loss: {meters[r_task_loss]:.6f}\tr-cps-loss: {meters[r_cps_loss]:.6f}\n'
-                                ).format(*a, meters=m))
-            if not self.args.is_epoch_lrer:
-                self.l_lrer.step()
-                self.r_lrer.step()
-        if self.args.is_epoch_lrer:
-            self.l_lrer.step()
-            self.r_lrer.step()
-
-    def _validate(self, data_loader, epoch):
-        self.meters.reset()
-        self.l_model.eval(); self.r_model.eval()
-        for idx, (inp, gt) in enumerate(data_loader):
-            inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
-            for mid, model, crit in (('l', self.l_model, self.l_criterion), ('r', self.r_model, self.r_criterion)):
-                resulter = model.forward(inp)[0]
-                pred = tool.dict_value(resulter, 'pred')
-                self.meters.update('{0}_task_loss'.format(mid), torch.mean(crit.forward(pred, gt, inp)).data)
-                self._metrics(resulter, gt, inp, mid)
-        self._log_validation_metrics(('l', 'r'))
-
-    def _save_checkpoint(self, epoch):
-        state = {'algorithm': self.NAME, 'epoch': epoch,
-                 'l_model': self.l_model.state_dict(), 'r_model': self.r_model.state_dict(),
-                 'l_optimizer': self.l_optimizer.state_dict(), 'r_optimizer': self.r_optimizer.state_dict(),
-                 'l_lrer': self.l_lrer.state_dict(), 'r_lrer': self.r_lrer.state_dict()}
-        torch.save(state, os.path.join(self.args.checkpoint_path, 'checkpoint_{0}.ckpt'.format(epoch)))
-
-    def _load_checkpoint(self):
-        checkpoint = torch.load(self.args.resume, weights_only=False)
-        name = tool.dict_value(checkpoint, 'algorithm', default='unknown')
-        if name != self.NAME:
-            logger.log_err('Unmatched SSL algorithm format in checkpoint => required: {0} - given: {1}\n'
-                           .format(self.NAME, name))
-        for key in ('l_model', 'r_model', 'l_optimizer', 'r_optimizer', 'l_lrer', 'r_lrer'):
-            getattr(self, key).load_state_dict(checkpoint[key])
-        self.l_model.arena.adopt_optimizer_state(self.l_optimizer)
-        self.r_model.arena.adopt_optimizer_state(self.r_optimizer)
-        return checkpoint['epoch']
+    def validate_step(self, inp, gt):
+        inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
+        for mid, model, crit in (('l', self.l_model, self.l_criterion), ('r', self.r_model, self.r_criterion)):
+            self._validate_model(model, crit, inp, gt, mid + '_task_loss', mid)

@@ -6,9 +6,6 @@ the unlabeled rows -> softmax -> mix of the two halves with the same mask (pseud
 batch-global confidence scalar -> student fwd on the mixed images -> fused softmax+MSE
 (confidence * rampup * cons_scale) -> backward -> SGD fused with the teacher EMA.
 Three separate forwards are kept (BN batch statistics depend on the grouping, SURVEY.md 7)."""
-import os
-import time
-
 import numpy as np
 import torch
 
@@ -73,6 +70,11 @@ class BoxMaskGenerator:
 class SSLCUTMIX(ssl_base._SSLBase):
     NAME = 'ssl_cutmix'
     SUPPORTED_TASK_TYPES = [CLASSIFICATION]
+    RAMPUP_EPOCHS = 'cons_rampup_epochs'
+    LOG_LINES = ('  student-{3}\t=>\t'
+                 's-task-loss: {meters[task_loss]:.6f}\t'
+                 's-cons-loss: {meters[cons_loss]:.6f}\n')
+    VALIDATION_IDS = ('student', 'teacher')
 
     def __init__(self, args):
         super().__init__(args)
@@ -157,55 +159,7 @@ class SSLCUTMIX(ssl_base._SSLBase):
         ema_decay = min(1 - 1 / (cur_step + 1), self.args.ema_decay)
         s_arena.sgd_step(self.s_optimizer, teacher=t_arena, ema_d=ema_decay)
 
-    def _train(self, data_loader, epoch):
-        self.meters.reset()
-        self.s_model.train()
-        self.t_model.train()
-        for idx, (inp, gt) in enumerate(ssl_base.device_prefetch(data_loader)):
-            timer = time.time()
-            cur_step = len(data_loader) * epoch + idx
-            total_steps = len(data_loader) * self.args.cons_rampup_epochs
-            self.train_step(inp, gt, cur_step, total_steps)
-            self.meters.update('batch_time', time.time() - timer)
-            if idx % self.args.log_freq == 0:
-                self._log_step(lambda m, a=(epoch + 1, idx, len(data_loader), self.args.task): ('step: [{0}][{1}/{2}]\tbatch-time: {meters[batch_time]:.3f}\n'
-                                '  student-{3}\t=>\t'
-                                's-task-loss: {meters[task_loss]:.6f}\t'
-                                's-cons-loss: {meters[cons_loss]:.6f}\n'
-                                ).format(*a, meters=m))
-            if not self.args.is_epoch_lrer:
-                self.s_lrer.step()
-        if self.args.is_epoch_lrer:
-            self.s_lrer.step()
-
-    def _validate(self, data_loader, epoch):
-        self.meters.reset()
-        self.s_model.eval()
-        self.t_model.eval()
-        for idx, (inp, gt) in enumerate(data_loader):
-            inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
-            for key, model, id_str in (('s', self.s_model, 'student'), ('t', self.t_model, 'teacher')):
-                resulter, _ = model.forward(inp)
-                pred = tool.dict_value(resulter, 'pred')
-                self.meters.update(key + '_task_loss', torch.mean(self.s_criterion.forward(pred, gt, inp)).data)
-                self._metrics(resulter, gt, inp, id_str)
-        self._log_validation_metrics(('student', 'teacher'))
-
-    def _save_checkpoint(self, epoch):
-        state = {'algorithm': self.NAME, 'epoch': epoch,
-                 's_model': self.s_model.state_dict(), 't_model': self.t_model.state_dict(),
-                 's_optimizer': self.s_optimizer.state_dict(), 's_lrer': self.s_lrer.state_dict()}
-        torch.save(state, os.path.join(self.args.checkpoint_path, 'checkpoint_{0}.ckpt'.format(epoch)))
-
-    def _load_checkpoint(self):
-        checkpoint = torch.load(self.args.resume, weights_only=False)
-        name = tool.dict_value(checkpoint, 'algorithm', default='unknown')
-        if name != self.NAME:
-            logger.log_err('Unmatched SSL algorithm format in checkpoint => required: {0} - given: {1}\n'
-                           .format(self.NAME, name))
-        self.s_model.load_state_dict(checkpoint['s_model'])
-        self.t_model.load_state_dict(checkpoint['t_model'])
-        self.s_optimizer.load_state_dict(checkpoint['s_optimizer'])
-        self.s_model.arena.adopt_optimizer_state(self.s_optimizer)
-        self.s_lrer.load_state_dict(checkpoint['s_lrer'])
-        return checkpoint['epoch']
+    def validate_step(self, inp, gt):
+        inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
+        self._validate_model(self.s_model, self.s_criterion, inp, gt, 's_task_loss', 'student')
+        self._validate_model(self.t_model, self.s_criterion, inp, gt, 't_task_loss', 'teacher')

@@ -7,9 +7,6 @@ flaw-correction loss both_bad * flawmap^2, dynamic-consistency MSE(softmax, dc_g
 (2) FD ground truth on the labeled rows (|onehot - softmax| -> blur -> nu x (dilate -> blur) ->
 min-max, the 179x179 depthwise convolutions of the reference run as separable 1-D passes),
 MSE, backward through the step-0 FD graphs, Adam(0.9, 0.99), PolynomialLR."""
-import os
-import time
-
 import torch
 import torch.nn as nn
 import torch.optim as optim
@@ -97,6 +94,14 @@ class FlawDetector(nn.Module):
 class SSLGCT(ssl_base._SSLBase):
     NAME = 'ssl_gct'
     SUPPORTED_TASK_TYPES = [REGRESSION, CLASSIFICATION]
+    RAMPUP_EPOCHS = 'dc_rampup_epochs'
+    LOG_LINES = ('  l-{3}\t=>\tl-task-loss: {meters[l_task_loss]:.6f}\tl-dc-loss: {meters[l_dc_loss]:.6f}\t'
+                 'l-fc-loss: {meters[l_fc_loss]:.6f}\n'
+                 '  r-{3}\t=>\tr-task-loss: {meters[r_task_loss]:.6f}\tr-dc-loss: {meters[r_dc_loss]:.6f}\t'
+                 'r-fc-loss: {meters[r_fc_loss]:.6f}\n'
+                 '  fd\t=>\tl-fd-loss: {meters[l_fd_loss]:.6f}\tr-fd-loss: {meters[r_fd_loss]:.6f}\n')
+    ITER_LRERS = ('fd_lrer',)
+    VALIDATION_IDS = ('l', 'r')
 
     def __init__(self, args):
         super().__init__(args)
@@ -218,61 +223,7 @@ class SSLGCT(ssl_base._SSLBase):
         self.fd_model.arena.all_reduce_grads()
         self.fd_model.arena.adam_step(self.fd_optimizer)
 
-    def _train(self, data_loader, epoch):
-        self.meters.reset()
-        self.l_model.train(); self.r_model.train(); self.fd_model.train()
-        for idx, (inp, gt) in enumerate(ssl_base.device_prefetch(data_loader)):
-            timer = time.time()
-            cur_steps = len(data_loader) * epoch + idx
-            total_steps = len(data_loader) * self.args.dc_rampup_epochs
-            self.train_step(inp, gt, cur_steps, total_steps)
-            self.meters.update('batch_time', time.time() - timer)
-            if idx % self.args.log_freq == 0:
-                self._log_step(lambda m, a=(epoch + 1, idx, len(data_loader), self.args.task): ('step: [{0}][{1}/{2}]\tbatch-time: {meters[batch_time]:.3f}\n'
-                                '  l-{3}\t=>\tl-task-loss: {meters[l_task_loss]:.6f}\tl-dc-loss: {meters[l_dc_loss]:.6f}\t'
-                                'l-fc-loss: {meters[l_fc_loss]:.6f}\n'
-                                '  r-{3}\t=>\tr-task-loss: {meters[r_task_loss]:.6f}\tr-dc-loss: {meters[r_dc_loss]:.6f}\t'
-                                'r-fc-loss: {meters[r_fc_loss]:.6f}\n'
-                                '  fd\t=>\tl-fd-loss: {meters[l_fd_loss]:.6f}\tr-fd-loss: {meters[r_fd_loss]:.6f}\n'
-                                ).format(*a, meters=m))
-            self.fd_lrer.step()
-            if not self.args.is_epoch_lrer:
-                self.l_lrer.step()
-                self.r_lrer.step()
-        if self.args.is_epoch_lrer:
-            self.l_lrer.step()
-            self.r_lrer.step()
-
-    def _validate(self, data_loader, epoch):
-        self.meters.reset()
-        self.l_model.eval(); self.r_model.eval(); self.fd_model.eval()
-        for idx, (inp, gt) in enumerate(data_loader):
-            inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
-            for mid, model, crit in (('l', self.l_model, self.l_criterion), ('r', self.r_model, self.r_criterion)):
-                resulter = model.forward(inp)[0]
-                pred = tool.dict_value(resulter, 'pred')
-                self.meters.update('{0}_task_loss'.format(mid), torch.mean(crit.forward(pred, gt, inp)).data)
-                self._metrics(resulter, gt, inp, mid)
-        self._log_validation_metrics(('l', 'r'))
-
-    def _save_checkpoint(self, epoch):
-        state = {'algorithm': self.NAME, 'epoch': epoch,
-                 'l_model': self.l_model.state_dict(), 'r_model': self.r_model.state_dict(),
-                 'fd_model': self.fd_model.state_dict(),
-                 'l_optimizer': self.l_optimizer.state_dict(), 'r_optimizer': self.r_optimizer.state_dict(),
-                 'fd_optimizer': self.fd_optimizer.state_dict(),
-                 'l_lrer': self.l_lrer.state_dict(), 'r_lrer': self.r_lrer.state_dict(), 'fd_lrer': self.fd_lrer.state_dict()}
-        torch.save(state, os.path.join(self.args.checkpoint_path, 'checkpoint_{0}.ckpt'.format(epoch)))
-
-    def _load_checkpoint(self):
-        checkpoint = torch.load(self.args.resume, weights_only=False)
-        name = tool.dict_value(checkpoint, 'algorithm', default='unknown')
-        if name != self.NAME:
-            logger.log_err('Unmatched SSL algorithm format in checkpoint => required: {0} - given: {1}\n'
-                           .format(self.NAME, name))
-        for key in ('l_model', 'r_model', 'fd_model', 'l_optimizer', 'r_optimizer', 'fd_optimizer', 'l_lrer', 'r_lrer', 'fd_lrer'):
-            getattr(self, key).load_state_dict(checkpoint[key])
-        self.l_model.arena.adopt_optimizer_state(self.l_optimizer)
-        self.r_model.arena.adopt_optimizer_state(self.r_optimizer)
-        self.fd_model.arena.adopt_optimizer_state(self.fd_optimizer)    # Adam moments + step count
-        return checkpoint['epoch']
+    def validate_step(self, inp, gt):
+        inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
+        for mid, model, crit in (('l', self.l_model, self.l_criterion), ('r', self.r_model, self.r_criterion)):
+            self._validate_model(model, crit, inp, gt, mid + '_task_loss', mid)

@@ -9,9 +9,6 @@ but: the consistency loss and its gradient come from ONE fused kernel launch (12
 the CE gradient is written by the CE forward launch, SGD+EMA is one kernel per LR group over the
 flat parameter arena, softmax ('activated_pred') is only materialised if something reads it, and
 multi-GPU is one process per GPU with a single NCCL gradient all-reduce."""
-import os
-import time
-
 import torch
 
 from .. import ops
@@ -40,6 +37,13 @@ def ssl_mt(args, model_dict, optimizer_dict, lrer_dict, criterion_dict, task_fun
 class SSLMT(ssl_base._SSLBase):
     NAME = 'ssl_mt'
     SUPPORTED_TASK_TYPES = [REGRESSION, CLASSIFICATION]
+    RAMPUP_EPOCHS = 'cons_rampup_epochs'
+    LOG_LINES = ('  student-{3}\t=>\t'
+                 's-task-loss: {meters[s_task_loss]:.6f}\t'
+                 's-cons-loss: {meters[cons_loss]:.6f}\n'
+                 '  teacher-{3}\t=>\t'
+                 't-task-loss: {meters[t_task_loss]:.6f}\n')
+    VALIDATION_IDS = ('student', 'teacher')
 
     def __init__(self, args):
         super().__init__(args)
@@ -115,29 +119,6 @@ class SSLMT(ssl_base._SSLBase):
         ema_decay = min(1 - 1 / (cur_step + 1), self.args.ema_decay)
         s_arena.sgd_step(self.s_optimizer, teacher=t_arena, ema_d=ema_decay)
 
-    def _train(self, data_loader, epoch):
-        self.meters.reset()
-        self.s_model.train()
-        self.t_model.train()
-        for idx, (inp, gt) in enumerate(ssl_base.device_prefetch(data_loader)):
-            timer = time.time()
-            cur_step = len(data_loader) * epoch + idx
-            total_steps = len(data_loader) * self.args.cons_rampup_epochs
-            self.train_step(inp, gt, cur_step, total_steps)
-            self.meters.update('batch_time', time.time() - timer)
-            if idx % self.args.log_freq == 0:
-                self._log_step(lambda m, a=(epoch + 1, idx, len(data_loader), self.args.task): ('step: [{0}][{1}/{2}]\tbatch-time: {meters[batch_time]:.3f}\n'
-                                '  student-{3}\t=>\t'
-                                's-task-loss: {meters[s_task_loss]:.6f}\t'
-                                's-cons-loss: {meters[cons_loss]:.6f}\n'
-                                '  teacher-{3}\t=>\t'
-                                't-task-loss: {meters[t_task_loss]:.6f}\n'
-                                ).format(*a, meters=m))
-            if not self.args.is_epoch_lrer:
-                self.s_lrer.step()
-        if self.args.is_epoch_lrer:
-            self.s_lrer.step()
-
     def _batch_prehandle(self, inp, gt, is_train):
         """ssl_mt.py:337-357: host -> HBM; while training the first input element gets independent
         Gaussian noise for the student and the teacher (``pxl_gaussian_noise`` in place on each device
@@ -152,44 +133,15 @@ class SSLMT(ssl_base._SSLBase):
             t_inp = s_inp
         return s_inp, t_inp, ssl_base.to_device(gt)
 
-    def _validate(self, data_loader, epoch):
-        self.meters.reset()
-        self.s_model.eval()
-        self.t_model.eval()
-        for idx, (inp, gt) in enumerate(data_loader):
-            s_inp, t_inp, gt = self._batch_prehandle(inp, gt, False)
-            s_resulter, _ = self.s_model.forward(s_inp)
-            s_pred = tool.dict_value(s_resulter, 'pred')
-            self.meters.update('s_task_loss', torch.mean(self.s_criterion.forward(s_pred, gt, s_inp)).data)
-            t_resulter, _ = self.t_model.forward(t_inp)
-            t_pred = tool.dict_value(t_resulter, 'pred')
-            self.meters.update('t_task_loss', torch.mean(self.s_criterion.forward(t_pred, gt, t_inp)).data)
-            cons_loss = ops.mse_consistency(s_pred[0], t_pred[0].detach(), self.args.cons_scale)
-            self.meters.update('cons_loss', cons_loss.data)
-            self._metrics(s_resulter, gt, s_inp, 'student')
-            self._metrics(t_resulter, gt, t_inp, 'teacher')
-        self._log_validation_metrics(('student', 'teacher'))
-
-    def _save_checkpoint(self, epoch):
-        state = {'algorithm': self.NAME, 'epoch': epoch,
-                 's_model': self.s_model.state_dict(), 't_model': self.t_model.state_dict(),
-                 's_optimizer': self.s_optimizer.state_dict(), 's_lrer': self.s_lrer.state_dict()}
-        torch.save(state, os.path.join(self.args.checkpoint_path, 'checkpoint_{0}.ckpt'.format(epoch)))
-
-    def _load_checkpoint(self):
-        checkpoint = torch.load(self.args.resume, weights_only=False)
-        name = tool.dict_value(checkpoint, 'algorithm', default='unknown')
-        if name != self.NAME:
-            logger.log_err('Unmatched SSL algorithm format in checkpoint => required: {0} - given: {1}\n'
-                           .format(self.NAME, name))
-        self.s_model.load_state_dict(checkpoint['s_model'])
-        self.t_model.load_state_dict(checkpoint['t_model'])
-        self.s_optimizer.load_state_dict(checkpoint['s_optimizer'])
-        self.s_model.arena.adopt_optimizer_state(self.s_optimizer)
-        self.s_lrer.load_state_dict(checkpoint['s_lrer'])
-        return checkpoint['epoch']
-
-    def _pred_err(self):
-        logger.log_err('In SSL_MT, the \'resulter\' dict returned by the task model should contain the following keys:\n'
-                       '   (1) \'pred\'\t=>\tunactivated task predictions\n'
-                       '   (2) \'activated_pred\'\t=>\tactivated task predictions\n')
+    def validate_step(self, inp, gt):
+        s_inp, t_inp, gt = self._batch_prehandle(inp, gt, False)
+        s_resulter, _ = self.s_model.forward(s_inp)
+        s_pred = tool.dict_value(s_resulter, 'pred')
+        self.meters.update('s_task_loss', torch.mean(self.s_criterion.forward(s_pred, gt, s_inp)).data)
+        t_resulter, _ = self.t_model.forward(t_inp)
+        t_pred = tool.dict_value(t_resulter, 'pred')
+        self.meters.update('t_task_loss', torch.mean(self.s_criterion.forward(t_pred, gt, t_inp)).data)
+        cons_loss = ops.mse_consistency(s_pred[0], t_pred[0].detach(), self.args.cons_scale)
+        self.meters.update('cons_loss', cons_loss.data)
+        self._metrics(s_resulter, gt, s_inp, 'student')
+        self._metrics(t_resulter, gt, t_inp, 'teacher')

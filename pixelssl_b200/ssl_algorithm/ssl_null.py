@@ -1,8 +1,5 @@
 """Supervised-only baseline (pixelssl/ssl_algorithm/ssl_null.py): forward, CE on the labeled
 rows, backward, SGD, per-iteration LR step (ssl_null.py:78-144)."""
-import os
-import time
-
 import torch
 
 from ..utils import REGRESSION, CLASSIFICATION, logger, tool
@@ -25,6 +22,7 @@ def ssl_null(args, model_dict, optimizer_dict, lrer_dict, criterion_dict, task_f
 class SSLNULL(ssl_base._SSLBase):
     NAME = 'ssl_null'
     SUPPORTED_TASK_TYPES = [REGRESSION, CLASSIFICATION]
+    LOG_LINES = '  task-{3}\t=>\ttask-loss: {meters[task_loss]:.6f}\t'
 
     def __init__(self, args):
         super().__init__(args)
@@ -45,61 +43,27 @@ class SSLNULL(ssl_base._SSLBase):
         if not (self.args.ignore_unlabeled and self.args.unlabeled_batch_size == 0):
             logger.log_err('SSL_NULL is a supervised-only algorithm\n'
                            'Please set ignore_unlabeled = True and unlabeled_batch_size = 0\n')
-        self.meters.reset()
+        super()._train(data_loader, epoch)
+
+    def train_step(self, inp, gt, cur_step, total_steps):
         lbs = self.args.labeled_batch_size
-        self.model.train()
         arena = self.model.arena
-        for idx, (inp, gt) in enumerate(ssl_base.device_prefetch(data_loader)):
-            timer = time.time()
-            inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
-            arena.zero_grad()
-            resulter, debugger = self.model.forward(inp)
-            if 'pred' not in resulter or 'activated_pred' not in resulter:
-                logger.log_err('In SSL_NULL, the \'resulter\' dict returned by the task model should '
-                               'contain the keys \'pred\' and \'activated_pred\'\n')
-            pred = tool.dict_value(resulter, 'pred')
-            l_pred = func.split_tensor_tuple(pred, 0, lbs)
-            l_gt = func.split_tensor_tuple(gt, 0, lbs)
-            l_inp = func.split_tensor_tuple(inp, 0, lbs)
-            task_loss = torch.mean(self.criterion.forward(l_pred, l_gt, l_inp))
-            self.meters.update('task_loss', task_loss.data)
-            task_loss.backward()
-            arena.all_reduce_grads()
-            arena.sgd_step(self.optimizer)
-            self.meters.update('batch_time', time.time() - timer)
-            if idx % self.args.log_freq == 0:
-                self._log_step(lambda m, a=(epoch + 1, idx, len(data_loader), self.args.task): ('step: [{0}][{1}/{2}]\tbatch-time: {meters[batch_time]:.3f}\n'
-                                '  task-{3}\t=>\ttask-loss: {meters[task_loss]:.6f}\t'
-                                ).format(*a, meters=m))
-            if not self.args.is_epoch_lrer:
-                self.lrer.step()
-        if self.args.is_epoch_lrer:
-            self.lrer.step()
+        inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
+        arena.zero_grad()
+        resulter, debugger = self.model.forward(inp)
+        if 'pred' not in resulter or 'activated_pred' not in resulter:
+            logger.log_err('In SSL_NULL, the \'resulter\' dict returned by the task model should '
+                           'contain the keys \'pred\' and \'activated_pred\'\n')
+        pred = tool.dict_value(resulter, 'pred')
+        l_pred = func.split_tensor_tuple(pred, 0, lbs)
+        l_gt = func.split_tensor_tuple(gt, 0, lbs)
+        l_inp = func.split_tensor_tuple(inp, 0, lbs)
+        task_loss = torch.mean(self.criterion.forward(l_pred, l_gt, l_inp))
+        self.meters.update('task_loss', task_loss.data)
+        task_loss.backward()
+        arena.all_reduce_grads()
+        arena.sgd_step(self.optimizer)
 
-    def _validate(self, data_loader, epoch):
-        self.meters.reset()
-        self.model.eval()
-        for idx, (inp, gt) in enumerate(data_loader):
-            inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
-            resulter, _ = self.model.forward(inp)
-            pred = tool.dict_value(resulter, 'pred')
-            self.meters.update('task_loss', torch.mean(self.criterion.forward(pred, gt, inp)).data)
-            self._metrics(resulter, gt, inp, 'task')
-        self._log_validation_metrics(('task',))
-
-    def _save_checkpoint(self, epoch):
-        state = {'algorithm': self.NAME, 'epoch': epoch, 'model': self.model.state_dict(),
-                 'optimizer': self.optimizer.state_dict(), 'lrer': self.lrer.state_dict()}
-        torch.save(state, os.path.join(self.args.checkpoint_path, 'checkpoint_{0}.ckpt'.format(epoch)))
-
-    def _load_checkpoint(self):
-        checkpoint = torch.load(self.args.resume, weights_only=False)
-        name = tool.dict_value(checkpoint, 'algorithm', default='unknown')
-        if name != self.NAME:
-            logger.log_err('Unmatched SSL algorithm format in checkpoint => required: {0} - given: {1}\n'
-                           .format(self.NAME, name))
-        self.model.load_state_dict(checkpoint['model'])
-        self.optimizer.load_state_dict(checkpoint['optimizer'])
-        self.model.arena.adopt_optimizer_state(self.optimizer)
-        self.lrer.load_state_dict(checkpoint['lrer'])
-        return checkpoint['epoch']
+    def validate_step(self, inp, gt):
+        inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
+        self._validate_model(self.model, self.criterion, inp, gt, 'task_loss', 'task')

@@ -7,9 +7,6 @@ launch per tensor instead of 2*bs slice assignments), the task model and the rot
 (ssl_s4l.py:381-400: two 4x4/2 convolutions + BatchNorm + LeakyReLU(0.2), global average pool, Linear -> 4) run
 forward, and three losses are summed: the task loss on the un-rotated labeled samples, ``rotated_sup_scale`` x the
 task loss on their rotated copies and ``rotation_scale`` x the cross entropy of the predicted quarter turn."""
-import os
-import time
-
 import numpy as np
 import torch
 import torch.nn as nn
@@ -132,11 +129,18 @@ class WrappedS4LModel(nn.Module):
 class SSLS4L(ssl_base._SSLBase):
     NAME = 'ssl_s4l'
     SUPPORTED_TASK_TYPES = [REGRESSION, CLASSIFICATION]
+    LOG_LINES = ('  task-{3}\t=>\t'
+                 'unrotated-task-loss: {meters[unrotated_task_loss]:.6f}\t'
+                 'rotated-task-loss: {meters[rotated_task_loss]:.6f}\n'
+                 '  rotation-{3}\t=>\t'
+                 'rotation-loss: {meters[rotation_loss]:.6f}\t'
+                 'rotation-acc: {meters[rotation_acc]:.6f}\n')
 
     def __init__(self, args):
         super().__init__(args)
         self.task_model = self.rotation_classifier = None
         self.model = self.optimizer = self.lrer = self.criterion = None
+        self._first_batch = True             # _inp_warn looks at the first batch of every epoch
         if self.args.rotation_scale < 0:
             logger.log_err('The argument - rotation_scale - is not set (or invalid)\n'
                            'Please set - rotation_scale >= 0 - for training\n')
@@ -169,8 +173,12 @@ class SSLS4L(ssl_base._SSLBase):
         self._algorithm_warn()
 
     # ------------------------------------------------------------------------------------------
-    def train_step(self, inp, gt):
+    def train_step(self, inp, gt, cur_step, total_steps):
         """Loop body of ssl_s4l.py:120-175 on (host or device) tuples ``inp`` / ``gt``."""
+        if self._first_batch:
+            self._first_batch = False
+            if len(gt) > 1:
+                self._inp_warn()
         original_lbs = int(self.args.labeled_batch_size / 2)
         original_bs = int(self.args.batch_size / 2)
         inp, gt = self._batch_prehandle(inp, gt, True)
@@ -203,60 +211,18 @@ class SSLS4L(ssl_base._SSLBase):
         self.meters.update('rotation_acc', rotation_acc[0])
 
     def _train(self, data_loader, epoch):
-        self.meters.reset()
-        self.model.train()
-        for idx, (inp, gt) in enumerate(ssl_base.device_prefetch(data_loader)):
-            timer = time.time()
-            if len(gt) > 1 and idx == 0:
-                self._inp_warn()
-            self.train_step(inp, gt)
-            self.meters.update('batch_time', time.time() - timer)
-            if idx % self.args.log_freq == 0:
-                self._log_step(lambda m, a=(epoch + 1, idx, len(data_loader), self.args.task): (
-                    'step: [{0}][{1}/{2}]\tbatch-time: {meters[batch_time]:.3f}\n'
-                    '  task-{3}\t=>\t'
-                    'unrotated-task-loss: {meters[unrotated_task_loss]:.6f}\t'
-                    'rotated-task-loss: {meters[rotated_task_loss]:.6f}\n'
-                    '  rotation-{3}\t=>\t'
-                    'rotation-loss: {meters[rotation_loss]:.6f}\t'
-                    'rotation-acc: {meters[rotation_acc]:.6f}\n').format(*a, meters=m))
-            if not self.args.is_epoch_lrer:
-                self.lrer.step()
-        if self.args.is_epoch_lrer:
-            self.lrer.step()
+        self._first_batch = True
+        super()._train(data_loader, epoch)
 
-    def _validate(self, data_loader, epoch):
-        self.meters.reset()
-        self.model.eval()
-        for idx, (inp, gt) in enumerate(data_loader):
-            inp, gt = self._batch_prehandle(inp, gt, False)
-            resulter, _ = self.model.forward(inp)
-            pred = tool.dict_value(resulter, 'pred')
-            pred_rotation = tool.dict_value(resulter, 'rotation')
-            self.meters.update('task_loss', torch.mean(self.criterion.forward(pred, gt[:-1], inp)).data)
-            rotation_loss = self.args.rotation_scale * torch.mean(self.rotation_criterion(pred_rotation, gt[-1]))
-            self.meters.update('rotation_loss', rotation_loss.data)
-            self._metrics(resulter, gt[:-1], inp, 'task')
-        self._log_validation_metrics(('task',))
-
-    def _save_checkpoint(self, epoch):
-        state = {'algorithm': self.NAME, 'epoch': epoch, 'model': self.model.state_dict(),
-                 'optimizer': self.optimizer.state_dict(), 'lrer': self.lrer.state_dict()}
-        torch.save(state, os.path.join(self.args.checkpoint_path, 'checkpoint_{0}.ckpt'.format(epoch)))
-
-    def _load_checkpoint(self):
-        checkpoint = torch.load(self.args.resume, weights_only=False)
-        name = tool.dict_value(checkpoint, 'algorithm', default='unknown')
-        if name != self.NAME:
-            logger.log_err('Unmatched ssl algorithm format in checkpoint => required: {0} - given: {1}\n'
-                           .format(self.NAME, name))
-        self.model.load_state_dict(checkpoint['model'])
-        self.optimizer.load_state_dict(checkpoint['optimizer'])
-        self.model.arena.adopt_optimizer_state(self.optimizer)
-        self.lrer.load_state_dict(checkpoint['lrer'])
-        self.task_model = self.model.module.task_model
-        self.rotation_classifier = self.model.module.rotation_classifier
-        return checkpoint['epoch']
+    def validate_step(self, inp, gt):
+        inp, gt = self._batch_prehandle(inp, gt, False)
+        resulter, _ = self.model.forward(inp)
+        pred = tool.dict_value(resulter, 'pred')
+        pred_rotation = tool.dict_value(resulter, 'rotation')
+        self.meters.update('task_loss', torch.mean(self.criterion.forward(pred, gt[:-1], inp)).data)
+        rotation_loss = self.args.rotation_scale * torch.mean(self.rotation_criterion(pred_rotation, gt[-1]))
+        self.meters.update('rotation_loss', rotation_loss.data)
+        self._metrics(resulter, gt[:-1], inp, 'task')
 
     # ------------------------------------------------------------------------------------------
     def _batch_prehandle(self, inp, gt, is_train):

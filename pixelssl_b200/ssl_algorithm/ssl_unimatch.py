@@ -22,8 +22,6 @@ Host draws, once per step and in this order:
   * the Dropout2d factors from torch's CPU generator, as CCT's DropOutDecoder draws them: one [n, C] tensor per
     feature map the task model perturbs (``fp_channels``), n = lbs + ubs."""
 import math
-import os
-import time
 
 import numpy as np
 import torch
@@ -118,6 +116,10 @@ def draw_fp_scales(n, channels, p):
 class SSLUNIMATCH(ssl_base._SSLBase):
     NAME = 'ssl_unimatch'
     SUPPORTED_TASK_TYPES = [CLASSIFICATION]
+    RAMPUP_EPOCHS = 'uni_rampup_epochs'
+    LOG_LINES = ('  task-{3}\t=>\ttask-loss: {meters[task_loss]:.6f}\ts1-loss: {meters[s1_loss]:.6f}\t'
+                 's2-loss: {meters[s2_loss]:.6f}\tfp-loss: {meters[fp_loss]:.6f}\t'
+                 'mask-ratio: {meters[mask_ratio]:.4f}\n')
 
     def __init__(self, args):
         super().__init__(args)
@@ -200,49 +202,6 @@ class SSLUNIMATCH(ssl_base._SSLBase):
         self.model.arena.all_reduce_grads()
         self.model.arena.sgd_step(self.optimizer)
 
-    def _train(self, data_loader, epoch):
-        self.meters.reset()
-        self.model.train()
-        for idx, (inp, gt) in enumerate(ssl_base.device_prefetch(data_loader)):
-            timer = time.time()
-            cur_step = len(data_loader) * epoch + idx
-            total_steps = len(data_loader) * self.args.uni_rampup_epochs
-            self.train_step(inp, gt, cur_step, total_steps)
-            self.meters.update('batch_time', time.time() - timer)
-            if idx % self.args.log_freq == 0:
-                self._log_step(lambda m, a=(epoch + 1, idx, len(data_loader), self.args.task): ('step: [{0}][{1}/{2}]\tbatch-time: {meters[batch_time]:.3f}\n'
-                                '  task-{3}\t=>\ttask-loss: {meters[task_loss]:.6f}\ts1-loss: {meters[s1_loss]:.6f}\t'
-                                's2-loss: {meters[s2_loss]:.6f}\tfp-loss: {meters[fp_loss]:.6f}\t'
-                                'mask-ratio: {meters[mask_ratio]:.4f}\n').format(*a, meters=m))
-            if not self.args.is_epoch_lrer:
-                self.lrer.step()
-        if self.args.is_epoch_lrer:
-            self.lrer.step()
-
-    def _validate(self, data_loader, epoch):
-        self.meters.reset()
-        self.model.eval()
-        for idx, (inp, gt) in enumerate(data_loader):
-            inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
-            resulter, _ = self.model.forward(inp)
-            pred = tool.dict_value(resulter, 'pred')
-            self.meters.update('task_loss', torch.mean(self.criterion.forward(pred, gt, inp)).data)
-            self._metrics(resulter, gt, inp, 'task')
-        self._log_validation_metrics(('task',))
-
-    def _save_checkpoint(self, epoch):
-        state = {'algorithm': self.NAME, 'epoch': epoch, 'model': self.model.state_dict(),
-                 'optimizer': self.optimizer.state_dict(), 'lrer': self.lrer.state_dict()}
-        torch.save(state, os.path.join(self.args.checkpoint_path, 'checkpoint_{0}.ckpt'.format(epoch)))
-
-    def _load_checkpoint(self):
-        checkpoint = torch.load(self.args.resume, weights_only=False)
-        name = tool.dict_value(checkpoint, 'algorithm', default='unknown')
-        if name != self.NAME:
-            logger.log_err('Unmatched SSL algorithm format in checkpoint => required: {0} - given: {1}\n'
-                           .format(self.NAME, name))
-        self.model.load_state_dict(checkpoint['model'])
-        self.optimizer.load_state_dict(checkpoint['optimizer'])
-        self.model.arena.adopt_optimizer_state(self.optimizer)
-        self.lrer.load_state_dict(checkpoint['lrer'])
-        return checkpoint['epoch']
+    def validate_step(self, inp, gt):
+        inp, gt = ssl_base.to_device(inp), ssl_base.to_device(gt)
+        self._validate_model(self.model, self.criterion, inp, gt, 'task_loss', 'task')
