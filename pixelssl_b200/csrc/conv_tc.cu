@@ -374,15 +374,20 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     // fp16 operands: the K loop of one tile.  It makes the adds of a loop that waits for every MMA group before it
     // adds, on the same MMA chains and in the same order, so its results are bit-identical to that loop's; only the
     // waits that order nothing are gone:
-    //   f16x3:  P1 part = hi*hi (k0,k1), C corr = lo*hi + hi*lo (k0..k3) | wait 1, acc += part        (C still runs)
-    //           P2 part = hi*hi (k2,k3)                                  | wait 0, acc += part + corr
+    //   f16x3:  P1 part = hi*hi (k0,k1) | acc += corr (the previous stage's part + corr)
+    //           C corr = lo*hi + hi*lo (k0..k3) | wait 1, acc += part                            (C still runs)
+    //           P2 part = hi*hi (k2,k3)         | wait 0, corr = part + corr
     //   f16:    P1 part = hi*hi (k0,k1) | wait 1, acc += corr (P2 of the previous stage)
     //           P2 corr = hi*hi (k2,k3) | wait 1, acc += part
-    // The last add of an f16x3 stage needs its second hi*hi half and its corrections in registers at once, and at
-    // BN = 128 there is no room for a fourth register tile (acc, part, corr take 192 of the 232 registers), so that
-    // wait empties the queue; the other consumer warpgroup covers the gap.  In f16 a stage is read until its last
-    // group completes, which the first wait of the next stage (or the tile's final wait) proves: its `empty` arrive
-    // comes then.  The ring stays as it was: at BN = 128 three 64 KB stages fill the shared memory.
+    // The last add of an f16x3 stage, acc += (part + corr), needs its second hi*hi half and its corrections in
+    // registers at once, and at BN = 128 there is no room for a fourth register tile (acc, part, corr take 192 of the
+    // 232 registers), so its wait empties this warpgroup's queue.  Only the inner sum is taken there; it frees `part`,
+    // and the outer add follows once the next stage's P1 is issued (or at the end of the tile), so the tensor pipe
+    // runs P1 during it.  The values and the order of the adds into acc are those of the one-line add.  The loop is
+    // not limited by operand delivery: loading no B_lo plane, a quarter of a stage's bytes, shortens it by under 1 %
+    // (DESIGN.md section 7).  In f16 a stage is read until its last group completes, which the first wait of the next
+    // stage (or the tile's final wait) proves: its `empty` arrive comes then.  The ring stays as it was: at BN = 128
+    // three 64 KB stages fill the shared memory.
     auto f16_tile = [&](auto split3_c) -> bool {
         constexpr bool S3 = decltype(split3_c)::value;
         uint32_t prev = 0;
@@ -399,6 +404,13 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             for (int k = 0; k < 2; ++k) wgmma_op<BN, 1>(part, da + 2 * k, db + 2 * k, k);
             wg_commit();
             if (S3) {
+                if (it > 0) {
+                    fence_regs(corr);
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) acc[i] += corr[i];     // the previous stage's last add
+                    wg_arrive();
+                    fence_regs(corr);
+                }
 #pragma unroll
                 for (int k = 0; k < 4; ++k) wgmma_op<BN, 1>(corr, dal + 2 * k, db + 2 * k, k);
 #pragma unroll
@@ -418,7 +430,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 fence_regs(corr);
                 mbar_arrive(&empty_bar[s]);
 #pragma unroll
-                for (int i = 0; i < BN / 2; ++i) acc[i] += part[i] + corr[i];
+                for (int i = 0; i < BN / 2; ++i) corr[i] = part[i] + corr[i];   // added into acc after the next P1
             } else {
                 asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
                 fence_regs(corr);
@@ -444,9 +456,9 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             wg_wait0();
             fence_regs(corr);
             mbar_arrive(&empty_bar[prev]);
-#pragma unroll
-            for (int i = 0; i < BN / 2; ++i) acc[i] += corr[i];
         }
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += corr[i];
         return true;
     };
     for (int tile = blockIdx.x; tile < p.total_tiles && ok; tile += gridDim.x) {
