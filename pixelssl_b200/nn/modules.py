@@ -98,6 +98,37 @@ class BatchNorm2d(nn.Module):
 SynchronizedBatchNorm2d = BatchNorm2d
 
 
+class LanePaddedBatchNorm:
+    """A BatchNorm2d applied to a map carried in ``lanes`` >= num_features channel lanes: the affine parameters are
+    zero-padded and the running statistics padded with mean 0 / variance 1, so the pad lanes stay exact zeros and take
+    no part in any gradient.  It has the attributes conv_bn_act and depthwise_bn_pair read; ``done()`` copies the
+    updated running statistics of the real channels back into the module (checkpoints keep the unpadded shapes)."""
+
+    def __init__(self, bn, lanes):
+        self.bn, self.pad = bn, lanes - bn.num_features
+        self.training, self.momentum, self.eps = bn.training, bn.momentum, bn.eps
+        self.sync_group, self.multi_replica_formula = bn.sync_group, bn.multi_replica_formula
+        if self.pad:
+            self.weight = nn.functional.pad(bn.weight, (0, self.pad))
+            self.bias = nn.functional.pad(bn.bias, (0, self.pad))
+            self.running_mean = torch.cat([bn.running_mean, bn.running_mean.new_zeros(self.pad)])
+            self.running_var = torch.cat([bn.running_var, bn.running_var.new_ones(self.pad)])
+        else:
+            self.weight, self.bias, self.running_mean, self.running_var = bn.weight, bn.bias, bn.running_mean, bn.running_var
+
+    def __call__(self, x, relu=False, residual=None):
+        return ops.bn_act(ops.as_cl(x), self.weight, self.bias, self.running_mean, self.running_var,
+                          training=self.training, momentum=self.momentum, eps=self.eps, relu=relu, residual=residual,
+                          group=self.sync_group if self.training else None, clamp_var=self.multi_replica_formula)
+
+    def done(self):
+        if self.pad and self.training:
+            n = self.bn.num_features
+            with torch.no_grad():
+                self.bn.running_mean.copy_(self.running_mean[:n])
+                self.bn.running_var.copy_(self.running_var[:n])
+
+
 # decoder building blocks shared by the PSPNet head (_pspnet.py:15-54) and the CCT decoders (ssl_cct.py:501-539)
 class PixelShuffle(nn.Module):
     """conv1x1 C -> 4C (bias, ICNR init) + ReLU + nn.PixelShuffle(2)."""

@@ -1262,34 +1262,59 @@ def _bn_train_forward(x, sums, rows, C, gamma, beta, running_mean, running_var, 
     return count
 
 
-def _bn_backward_sums(dsums, C, gamma, beta, group):
-    """Train-mode (Sync)BN backward after its reduce launch.  d(gamma), d(beta) come from the LOCAL sums (data
-    parallelism averages them with the other gradients).  When the gradient arena is in place they are accumulated by a
-    launch that runs anyway: the dx launch (single GPU) or the peer exchange (before it exchanges the sums); otherwise a
-    params launch writes them into tensors returned to autograd.  Then ``dsums`` is all-reduced over ``group``.
-    -> (dgamma, dbeta, gamma_acc, beta_acc): the tensors for autograd (None when accumulated in place) and the
-    accumulators the dx launch adds into (None unless it does)."""
-    grads_in_arena = (gamma.grad is not None and beta.grad is not None
-                      and gamma.grad.is_contiguous() and beta.grad.is_contiguous())
-    px = _peer_exchanges.get(id(group)) if group is not None else None
+H16_DX_TARGET_LOG2 = 12         # bn_bwd_dx: max|gamma*invstd| * absmax(dz) -> <= 2^12, 3 bits of headroom for the mean terms
+
+
+def _bn_backward(x, dy, coeff, gamma, beta, count, rows, C, relu, group, training=True, y=None, mask=None,
+                 want_dres=False, dx_pair=False, want_lo=True):
+    """(Sync)BN (+residual) (+ReLU) backward of a BN node with input ``x`` -> (dx, dres, dgamma, dbeta): a reduce
+    launch (sum dz, sum dz * xhat), the parameter gradients, then a dx launch.  y / mask: the ReLU mask source of both
+    launches (the fp32 result, or one byte per 4 values), else it is recomputed from x.  want_dres: dres = dz, the
+    gradient of the residual.  dx_pair: dx is written only as an fp16 pair (with its lo plane when want_lo) under a
+    device-side power-of-two scale and returned as an H16, else as an fp32 tensor.
+
+    Train mode: d(gamma), d(beta) come from the LOCAL sums (data parallelism averages them with the other gradients).
+    When the gradient arena is in place they are accumulated by a launch that runs anyway: the dx launch (single GPU)
+    or the peer exchange (before it exchanges the sums), and dgamma / dbeta are None; otherwise a params launch writes
+    them into tensors returned to autograd.  Then the sums are all-reduced over ``group``.
+    Eval mode (F.batch_norm(training=False) backward): dx = dz * gamma / sqrt(running_var + eps), d(gamma) = sum dz *
+    xhat, d(beta) = sum dz with xhat from the running statistics.  The params launch writes the parameter gradients;
+    the dx launch runs with zero batch sums, which removes its mean terms."""
+    dev = dy.device
+    dsums = _stat_zeros(2 * C, dev)
+    slot = _scale_slot(dev) if dx_pair else None
+    call('pxl_bn_bwd_reduce', _p(x), _p(y), _p(dy), _p(coeff[0]), _p(coeff[1]), int(relu), rows, C, _p(dsums),
+         _p(coeff[2]), _p(coeff[3]), _p(slot), _p(mask), _stream())
+    px = _peer_exchanges.get(id(group)) if (training and group is not None) else None
     if px is not None and 2 * C > _PEER_MAX_VALUES:
         px = None
-    acc_inplace = grads_in_arena and group is None
-    acc_in_exchange = grads_in_arena and px is not None
+    in_arena = (training and (group is None or px is not None) and gamma.grad is not None and beta.grad is not None
+                and gamma.grad.is_contiguous() and beta.grad.is_contiguous())
     dgamma = dbeta = None
-    if not (acc_inplace or acc_in_exchange):
-        dgamma = torch.empty(C, dtype=torch.float32, device=dsums.device)
-        dbeta = torch.empty(C, dtype=torch.float32, device=dsums.device)
+    if not in_arena:
+        dgamma = torch.empty(C, dtype=torch.float32, device=dev)
+        dbeta = torch.empty(C, dtype=torch.float32, device=dev)
         call('pxl_bn_bwd_params', _p(dsums), C, _p(dgamma), _p(dbeta), 0, _stream())
-    if group is not None:
-        if px is not None:
-            px.allreduce_bn(dsums, param_grads=(gamma.grad, beta.grad) if acc_in_exchange else None)
-        else:
-            import torch.distributed as dist
-            dist.all_reduce(dsums, group=group)
-    if acc_inplace:
-        return dgamma, dbeta, gamma.grad, beta.grad
-    return dgamma, dbeta, None, None
+    if not training:
+        dsums = _stat_zeros(2 * C, dev)
+    elif px is not None:
+        px.allreduce_bn(dsums, param_grads=(gamma.grad, beta.grad) if in_arena else None)
+    elif group is not None:
+        import torch.distributed as dist
+        dist.all_reduce(dsums, group=group)
+    gacc, bacc = (gamma.grad, beta.grad) if (in_arena and group is None) else (None, None)
+    if dx_pair:
+        n = rows * C
+        dpair = torch.empty((2, n), dtype=torch.float16, device=dev)
+        dx, out = H16(dpair, n, None, slot, want_lo), None
+        h16_out = (_p(dpair[0]), _p(dpair[1] if want_lo else None), _p(slot), H16_DX_TARGET_LOG2)
+    else:
+        dx = out = torch.empty_like(x)
+        h16_out = (None, None, None, 0)
+    dres = torch.empty_like(x) if want_dres else None
+    call('pxl_bn_bwd_dx', _p(x), _p(y), _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, int(relu),
+         _p(out), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc), *h16_out, _p(mask), _stream())
+    return dx, dres, dgamma, dbeta
 
 
 class _BnAct(torch.autograd.Function):
@@ -1324,6 +1349,7 @@ class _BnAct(torch.autograd.Function):
                 coeff[1].copy_(torch.rsqrt(running_var + eps))
             call('pxl_bn_apply', _p(x), _p(coeff[2]), _p(coeff[3]), _p(residual), int(relu), _p(y), rows, C,
                  None, None, 1.0, None, _stream())
+        # ReLU without residual: the backward recomputes the mask from x (same fmaf as the forward) instead of reading y
         ctx.save_for_backward(x, y if (relu and residual is not None) else None, gamma, coeff, running_var, beta)
         ctx.meta = (rows, C, count, bool(relu), residual is not None, bool(training), float(eps), group)
         return y
@@ -1332,28 +1358,8 @@ class _BnAct(torch.autograd.Function):
     def backward(ctx, dy):
         x, y, gamma, coeff, running_var, beta = ctx.saved_tensors
         rows, C, count, relu, has_res, training, eps, group = ctx.meta
-        dy = as_cl(dy)
-        dev = dy.device
-        dsums = _stat_zeros(2 * C, dev)
-        # ReLU without residual: the mask is recomputed from x (same fmaf as the forward) instead of reading y
-        ymask = y if (relu and has_res) else None
-        call('pxl_bn_bwd_reduce', _p(x), _p(ymask), _p(dy), _p(coeff[0]), _p(coeff[1]), int(relu), rows, C, _p(dsums),
-             _p(coeff[2]), _p(coeff[3]), None, None, _stream())
-        if not training:
-            # F.batch_norm(training=False) backward: dx = dz * gamma / sqrt(running_var + eps), d(gamma) = sum dz * xhat,
-            # d(beta) = sum dz with xhat from the running statistics.  The reduce launch gives the parameter sums; the
-            # dx launch runs with zero batch sums, which removes its mean terms.
-            dgamma = torch.empty(C, dtype=torch.float32, device=dev)
-            dbeta = torch.empty(C, dtype=torch.float32, device=dev)
-            call('pxl_bn_bwd_params', _p(dsums), C, _p(dgamma), _p(dbeta), 0, _stream())
-            dsums, gacc, bacc = _stat_zeros(2 * C, dev), None, None
-        else:
-            dgamma, dbeta, gacc, bacc = _bn_backward_sums(dsums, C, gamma, beta, group)
-        dx = torch.empty_like(x)
-        dres = torch.empty_like(x) if has_res else None
-        call('pxl_bn_bwd_dx', _p(x), _p(ymask), _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, int(relu),
-             _p(dx), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc), None, None, None, 0, None,
-             _stream())
+        dx, dres, dgamma, dbeta = _bn_backward(x, as_cl(dy), coeff, gamma, beta, count, rows, C, relu, group, training,
+                                               y=y, want_dres=has_res)
         return dx, dgamma, dbeta, None, None, dres, None, None, None, None, None, None, None
 
 
@@ -1371,8 +1377,6 @@ def bn_act(x, gamma, beta, running_mean, running_var, training=True, momentum=0.
 # ------------------------------------------------------------------------------------------------
 
 _residual_stash = {}            # block key -> gradient of the residual branch waiting for the block's first dgrad (one step)
-H16_DX_TARGET_LOG2 = 12         # bn_bwd_dx: max|gamma*invstd| * absmax(dz) -> <= 2^12, 3 bits of headroom for the mean terms
-_unit_out_pair = None           # H16 of the last _ConvBnAct.forward output (picked up by conv_bn_act right after apply)
 
 
 def _attach_pair(t, h, carrier=False):
@@ -1402,7 +1406,6 @@ class _ConvBnAct(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, residual, stride, padding, dilation,
                 momentum, eps, relu, group, clamp_var, out_mode, stash_key=None, stash_role=None):
-        global _unit_out_pair
         ctx.stash = (stash_key, stash_role)
         prec = _conv_precision
         want_lo = prec == 3
@@ -1433,10 +1436,10 @@ class _ConvBnAct(torch.autograd.Function):
         ctx.save_for_backward(xh.buf, weight, c, mask, gamma, coeff, beta)
         ctx.meta = (taps, N, H, W, Cin, OH, OW, Cout, stride, kh * kw, count, bool(relu), residual is not None, group,
                     xh.scale, want_lo, prec)
-        _unit_out_pair = H16(pair, n, H16_ACT_SCALE, None, want_lo) if pair is not None else None
-        if out_mode == 'pair':
-            return pair.view(torch.float32).view(N, OH, OW, Cout).permute(0, 3, 1, 2)
-        return y
+        out = pair.view(torch.float32).view(N, OH, OW, Cout).permute(0, 3, 1, 2) if out_mode == 'pair' else y
+        if pair is not None:
+            _attach_pair(out, H16(pair, n, H16_ACT_SCALE, None, want_lo), carrier=out_mode == 'pair')
+        return out
 
     @staticmethod
     def backward(ctx, dy):
@@ -1444,24 +1447,10 @@ class _ConvBnAct(torch.autograd.Function):
         taps, N, H, W, Cin, OH, OW, Cout, stride, T, count, relu, has_res, group, xscale, want_lo, prec = ctx.meta
         if is_carrier(dy):
             raise RuntimeError('gradient tensors are never fp16-pair carriers')
-        dy = as_cl(dy)
-        dev = dy.device
-        rows = N * OH * OW
-        n = rows * Cout
-        C = Cout
-        dsums = _stat_zeros(2 * C, dev)
-        slot = _scale_slot(dev)
         if relu and has_res and mask is None:
             raise RuntimeError('the ReLU mask of a residual unit was not recorded in the forward')
-        call('pxl_bn_bwd_reduce', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), int(relu), rows, C, _p(dsums),
-             _p(coeff[2]), _p(coeff[3]), _p(slot), _p(mask), _stream())
-        dgamma, dbeta, gacc, bacc = _bn_backward_sums(dsums, C, gamma, beta, group)
-        dpair = torch.empty((2, n), dtype=torch.float16, device=dev)
-        dres = torch.empty_like(c) if has_res else None
-        call('pxl_bn_bwd_dx', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, int(relu),
-             _p(None), _p(dres), rows, C, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc),
-             _p(dpair[0]), _p(dpair[1] if want_lo else None), _p(slot), H16_DX_TARGET_LOG2, _p(mask), _stream())
-        dh = H16(dpair, n, None, slot, want_lo)
+        dh, dres, dgamma, dbeta = _bn_backward(c, as_cl(dy), coeff, gamma, beta, count, N * OH * OW, Cout, relu, group,
+                                               mask=mask, want_dres=has_res, dx_pair=True, want_lo=want_lo)
         dx = dw = None
         stash_key, stash_role = ctx.stash
         if stash_role == 'give' and dres is not None:
@@ -1514,16 +1503,11 @@ def conv_bn_act(x, conv, bn, relu=False, residual=None, out_mode='both', stash_k
     stash_key / stash_role: a bottleneck whose residual branch is its own input marks its last unit 'give' and its
     first unit 'take' with a common key - the residual gradient then reaches the block input through the first
     unit's dgrad epilogue (out += ...) instead of through autograd's add."""
-    global _unit_out_pair
     if not is_carrier(x):
         x = as_cl(x)
-    out = _ConvBnAct.apply(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, residual,
-                           int(conv.stride), int(conv.padding), int(conv.dilation), float(bn.momentum), float(bn.eps),
-                           bool(relu), bn.sync_group, bool(bn.multi_replica_formula), out_mode, stash_key, stash_role)
-    pair, _unit_out_pair = _unit_out_pair, None
-    if pair is not None:
-        _attach_pair(out, pair, carrier=(out_mode == 'pair'))
-    return out
+    return _ConvBnAct.apply(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, residual,
+                            int(conv.stride), int(conv.padding), int(conv.dilation), float(bn.momentum), float(bn.eps),
+                            bool(relu), bn.sync_group, bool(bn.multi_replica_formula), out_mode, stash_key, stash_role)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1599,7 +1583,6 @@ class _DwBnPair(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, stride, dilation, momentum, eps, group, clamp_var):
-        global _unit_out_pair
         want_lo = _conv_precision == 3
         c, meta = _dw_forward(x, weight, stride, dilation)
         N, ld, H, W, C, OH, OW = meta[:7]
@@ -1614,23 +1597,15 @@ class _DwBnPair(torch.autograd.Function):
                                   (_p(pair[0]), _p(pair[1] if want_lo else None), float(H16_ACT_SCALE), None))
         ctx.save_for_backward(x, weight, c, gamma, coeff, beta)
         ctx.meta, ctx.bn = meta, (count, group)
-        _unit_out_pair = H16(pair, n, H16_ACT_SCALE, None, want_lo)
-        return pair.view(torch.float32).view(N, OH, OW, ld).permute(0, 3, 1, 2)
+        return _attach_pair(pair.view(torch.float32).view(N, OH, OW, ld).permute(0, 3, 1, 2),
+                            H16(pair, n, H16_ACT_SCALE, None, want_lo), carrier=True)
 
     @staticmethod
     def backward(ctx, dy):
         x, weight, c, gamma, coeff, beta = ctx.saved_tensors
         count, group = ctx.bn
         N, ld, H, W, C, OH, OW = ctx.meta[:7]
-        dy = as_cl(dy)
-        rows, dev = N * OH * OW, dy.device
-        dsums = _stat_zeros(2 * ld, dev)
-        call('pxl_bn_bwd_reduce', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), 0, rows, ld, _p(dsums),
-             _p(coeff[2]), _p(coeff[3]), None, None, _stream())
-        dgamma, dbeta, gacc, bacc = _bn_backward_sums(dsums, ld, gamma, beta, group)
-        dc = torch.empty_like(c)
-        call('pxl_bn_bwd_dx', _p(c), None, _p(dy), _p(coeff[0]), _p(coeff[1]), _p(gamma), _p(dsums), count, 0,
-             _p(dc), None, rows, ld, _p(coeff[2]), _p(coeff[3]), _p(gacc), _p(bacc), None, None, None, 0, None, _stream())
+        dc, _, dgamma, dbeta = _bn_backward(c, as_cl(dy), coeff, gamma, beta, count, N * OH * OW, ld, False, group)
         dx, dw = _dw_backward(x, weight, dc, ctx.meta, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
         return (dx, dw, dgamma, dbeta) + (None,) * 8
 
@@ -1638,11 +1613,8 @@ class _DwBnPair(torch.autograd.Function):
 def depthwise_bn_pair(x, weight, bn, stride=1, dilation=1):
     """depthwise_conv -> bn (train mode, the BatchNorm2d or a lane-padded view of it with the same attributes) as the
     fp16-pair carrier a following conv_bn_act unit reads; see _DwBnPair."""
-    global _unit_out_pair
-    out = _DwBnPair.apply(x, weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, int(stride), int(dilation),
-                          float(bn.momentum), float(bn.eps), bn.sync_group, bool(bn.multi_replica_formula))
-    pair, _unit_out_pair = _unit_out_pair, None
-    return _attach_pair(out, pair, carrier=True)
+    return _DwBnPair.apply(x, weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, int(stride), int(dilation),
+                           float(bn.momentum), float(bn.eps), bn.sync_group, bool(bn.multi_replica_formula))
 
 
 class _MaxPool(torch.autograd.Function):

@@ -16,7 +16,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .... import ops
-from ....nn.modules import Conv2d, BatchNorm2d
+from ....nn.modules import Conv2d, BatchNorm2d, LanePaddedBatchNorm
 from .resnet import build_backbone
 from .xception import AlignedXception
 
@@ -90,19 +90,10 @@ class _Reduce(_ConvBnReLU):
     parameters are zero, so the extra lanes hold exact zeros and take no part in any gradient."""
 
     def forward(self, x):
-        conv, bn = self[0], self[1]
-        pad = REDUCE_LANES - conv.out_channels
-        w = F.pad(conv.weight, (0, 0, 0, 0, 0, 0, 0, pad)).contiguous(memory_format=torch.channels_last)
-        y = ops.conv2d(ops.as_cl(x), w, None, want_bn_stats=bn.training)
-        gamma, beta = F.pad(bn.weight, (0, pad)), F.pad(bn.bias, (0, pad))
-        rm = torch.cat([bn.running_mean, bn.running_mean.new_zeros(pad)])
-        rv = torch.cat([bn.running_var, bn.running_var.new_ones(pad)])
-        out = ops.bn_act(y, gamma, beta, rm, rv, training=bn.training, momentum=bn.momentum, eps=bn.eps, relu=True,
-                         group=bn.sync_group if bn.training else None, clamp_var=bn.multi_replica_formula)
-        if bn.training:
-            with torch.no_grad():
-                bn.running_mean.copy_(rm[:conv.out_channels])
-                bn.running_var.copy_(rv[:conv.out_channels])
+        conv, bn = self[0], LanePaddedBatchNorm(self[1], REDUCE_LANES)
+        w = F.pad(conv.weight, (0, 0, 0, 0, 0, 0, 0, bn.pad)).contiguous(memory_format=torch.channels_last)
+        out = bn(ops.conv2d(ops.as_cl(x), w, None, want_bn_stats=bn.training), relu=True)
+        bn.done()
         return out
 
 

@@ -22,7 +22,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .... import ops
-from ....nn.modules import Conv2d, BatchNorm2d, DepthwiseConv2d
+from ....nn.modules import Conv2d, BatchNorm2d, DepthwiseConv2d, LanePaddedBatchNorm
 from .resnet import load_complete_state_dict
 
 CL = torch.channels_last
@@ -42,37 +42,9 @@ def _conv_view(conv, cin, cout):
                                  stride=conv.stride, padding=conv.padding, dilation=conv.dilation)
 
 
-class _BnView:
-    """bn with its affine parameters zero-padded and its running statistics padded with mean 0 / variance 1 to
-    ``lanes``; ``done()`` copies the updated running statistics of the real channels back into bn."""
-
-    def __init__(self, bn, lanes_):
-        self.bn, self.pad = bn, lanes_ - bn.num_features
-        self.training, self.momentum, self.eps = bn.training, bn.momentum, bn.eps
-        self.sync_group, self.multi_replica_formula = bn.sync_group, bn.multi_replica_formula
-        if self.pad:
-            self.weight, self.bias = F.pad(bn.weight, (0, self.pad)), F.pad(bn.bias, (0, self.pad))
-            self.running_mean = torch.cat([bn.running_mean, bn.running_mean.new_zeros(self.pad)])
-            self.running_var = torch.cat([bn.running_var, bn.running_var.new_ones(self.pad)])
-        else:
-            self.weight, self.bias, self.running_mean, self.running_var = bn.weight, bn.bias, bn.running_mean, bn.running_var
-
-    def __call__(self, x, relu=False, residual=None):
-        return ops.bn_act(ops.as_cl(x), self.weight, self.bias, self.running_mean, self.running_var,
-                          training=self.training, momentum=self.momentum, eps=self.eps, relu=relu, residual=residual,
-                          group=self.sync_group if self.training else None, clamp_var=self.multi_replica_formula)
-
-    def done(self):
-        if self.pad and self.training:
-            n = self.bn.num_features
-            with torch.no_grad():
-                self.bn.running_mean.copy_(self.running_mean[:n])
-                self.bn.running_var.copy_(self.running_var[:n])
-
-
 def _conv_bn(x, conv, bn, cin, cout, relu, residual=None):
     """relu?(bn(conv(x)) + residual) on lane-padded maps: one fused unit on the fp16-pair path, else conv2d + bn_act."""
-    cv, bv = _conv_view(conv, cin, cout), _BnView(bn, cout)
+    cv, bv = _conv_view(conv, cin, cout), LanePaddedBatchNorm(bn, cout)
     if ops.conv_bn_unit_ok(cv, bv):
         y = ops.conv_bn_act(x, cv, bv, relu=relu, residual=residual, out_mode='fp32')
     else:
@@ -96,7 +68,8 @@ class SeparableConv2d(nn.Module):
         """relu?(bn(self(x)) + residual): ``bn`` is the BatchNorm that follows this convolution in the tree.  On the
         fp16-pair path the depthwise BN's apply writes the pair the pointwise unit reads."""
         cin, cout = lanes(self.conv1.in_channels), lanes(self.pointwise.out_channels)
-        pw, bin_, bout = _conv_view(self.pointwise, cin, cout), _BnView(self.bn, cin), _BnView(bn, cout)
+        pw = _conv_view(self.pointwise, cin, cout)
+        bin_, bout = LanePaddedBatchNorm(self.bn, cin), LanePaddedBatchNorm(bn, cout)
         if ops.conv_bn_unit_ok(pw, bout):
             h = ops.depthwise_bn_pair(x, self.conv1.weight, bin_, self.conv1.stride, self.conv1.dilation)
             y = ops.conv_bn_act(h, pw, bout, relu=relu, residual=residual, out_mode='fp32')
@@ -193,7 +166,7 @@ class AlignedXception(nn.Module):
     def forward_low_level(self, img):
         """-> (low-level features [N,128,H/4,W/4] after block1's ReLU, the 2048-channel output at stride OS)."""
         w1 = F.pad(self.conv1.weight, (0, 0, 0, 0, 0, 0, 0, 64 - 32)).contiguous(memory_format=CL)
-        b1 = _BnView(self.bn1, 64)
+        b1 = LanePaddedBatchNorm(self.bn1, 64)
         x = b1(ops.stem_conv(img, w1, want_bn_stats=self.training), relu=True)        # 32 channels in 64 lanes
         b1.done()
         x = _conv_bn(x, self.conv2, self.bn2, 64, 64, True)
