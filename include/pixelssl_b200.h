@@ -228,7 +228,10 @@ int pxl_maxpool3x3s2_bwd(const float* x, const float* y, const float* dy, float*
  *   forward conv: mul=stride, div=1, dy_t = r*dil - pad.   dgrad: mul=1, div=stride, taps negated,
  *   weights transposed to [Cin][tap][Cout] (pxl_conv_transpose_weights).
  * precision: 0 = fp32 FFMA (exact fp32 accumulate), 1 = tf32 tensor cores (wgmma), 2 = 3xTF32
- *   error-compensated wgmma.  Unsupported (shape, precision) combos return PXL_ERR_UNSUPPORTED.
+ *   error-compensated wgmma, 3 / 4 = fp16-pair / single-fp16 wgmma.  pxl_conv_nhwc / pxl_conv_wgrad_nhwc are the
+ *   FFMA kernels and take precision 0 only (PXL_ERR_BAD_ARG otherwise); the wgmma kernels are launched through
+ *   pxl_conv_tc_launch_ex / pxl_conv_wgrad_tc_launch (1, 2) and the _h16_ entry points (3, 4).  Unsupported
+ *   shapes return PXL_ERR_UNSUPPORTED.
  * ------------------------------------------------------------------------------------------- */
 typedef struct {
     int N, H, W, Cin;        /* input tensor  */

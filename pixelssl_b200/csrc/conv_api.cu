@@ -1,23 +1,19 @@
-// Precision dispatch for the convolution entry points of include/pixelssl_b200.h.
+// The FFMA convolution entry points of include/pixelssl_b200.h; the wgmma kernels have entry points of their own.
 #include "common.cuh"
 
 extern "C" int pxl_conv_fp32_impl(const pxl_conv_geom*, const int*, const float*, const float*, const float*, float*, void*);
 extern "C" int pxl_conv_wgrad_fp32_impl(const pxl_conv_geom*, const int*, const float*, const float*, float*, void*);
-extern "C" int pxl_conv_tc_impl(const pxl_conv_geom*, const int*, const float*, const float*, const float*, float*, void*);
-extern "C" int pxl_conv_wgrad_tc_impl(const pxl_conv_geom*, const int*, const float*, const float*, float*, void*);
 
 extern "C" int pxl_conv_nhwc(const pxl_conv_geom* geom, const int* taps, const float* in, const float* w,
                              const float* bias, float* out, void* stream) {
-    if (!geom) return PXL_ERR_BAD_ARG;
-    if (geom->precision == 0) return pxl_conv_fp32_impl(geom, taps, in, w, bias, out, stream);
-    return pxl_conv_tc_impl(geom, taps, in, w, bias, out, stream);
+    if (!geom || geom->precision != 0) return PXL_ERR_BAD_ARG;
+    return pxl_conv_fp32_impl(geom, taps, in, w, bias, out, stream);
 }
 
 extern "C" int pxl_conv_wgrad_nhwc(const pxl_conv_geom* geom, const int* taps, const float* in,
                                    const float* dy, float* dw, void* stream) {
-    if (!geom) return PXL_ERR_BAD_ARG;
-    if (geom->precision == 0) return pxl_conv_wgrad_fp32_impl(geom, taps, in, dy, dw, stream);
-    return pxl_conv_wgrad_tc_impl(geom, taps, in, dy, dw, stream);
+    if (!geom || geom->precision != 0) return PXL_ERR_BAD_ARG;
+    return pxl_conv_wgrad_fp32_impl(geom, taps, in, dy, dw, stream);
 }
 
 // Scratch buffers of the kernels that store per-block partials and sum them in a fixed order, one per (purpose,

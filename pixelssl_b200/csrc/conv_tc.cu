@@ -796,14 +796,6 @@ extern "C" int pxl_conv_tc_status(void) {
     return v;
 }
 
-extern "C" int pxl_conv_tc_impl(const pxl_conv_geom* g, const int* taps, const float* in, const float* w,
-                                const float* bias, float* out, void* stream) {
-    if (!g) return PXL_ERR_BAD_ARG;
-    if (g->precision == 2) return PXL_ERR_UNSUPPORTED;     // 3xTF32 needs the split operands: pxl_conv_tc_launch_ex
-    if (g->precision > 2) return PXL_ERR_BAD_ARG;          // fp16 operands go through pxl_conv_h16_launch
-    return conv_tc_launch_core(g, taps, nullptr, in, nullptr, w, nullptr, bias, out, stream);
-}
-
 // ==========================================================================================
 // wgrad on wgmma:  dW[co][tap][ci] += sum_pixels dY[pix][co] * X[pix + tap][ci]
 //
@@ -1230,11 +1222,4 @@ static int conv_wgrad_tc_core(const pxl_conv_geom* g, const int* taps, const voi
     if (BN == 128) return launch_wgrad<128, 0>(mDy, mDyLo, mX, mXLo, p, grid, smem, st, dw, oscale_ptr);
     if (BN == 64) return launch_wgrad<64, 0>(mDy, mDyLo, mX, mXLo, p, grid, smem, st, dw, oscale_ptr);
     return launch_wgrad<32, 0>(mDy, mDyLo, mX, mXLo, p, grid, smem, st, dw, oscale_ptr);
-}
-
-extern "C" int pxl_conv_wgrad_tc_impl(const pxl_conv_geom* g, const int* taps, const float* in, const float* dy,
-                                      float* dw, void* stream) {
-    if (!g) return PXL_ERR_BAD_ARG;
-    if (g->precision == 2) return PXL_ERR_UNSUPPORTED;     // needs split operands: pxl_conv_wgrad_tc_launch
-    return pxl_conv_wgrad_tc_launch(g, taps, in, nullptr, dy, nullptr, dw, stream);
 }

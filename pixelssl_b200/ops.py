@@ -740,11 +740,17 @@ def h16_status_sites():
     return tuple(int(v) for v in out)
 
 
+def h16_has_lo(precision):
+    """Whether the fp16 pairs of a precision mode carry their lo plane: f16x3 (3) does, single fp16 (4) does not."""
+    return precision == 3
+
+
 def _pair_of(t, want_lo, scale=H16_ACT_SCALE):
-    """The fp16 pair of t: attached by its producer (same step, unmodified), else split now and memoised on t for the
-    step (an activation feeding several convolutions, a weight used by several launches)."""
+    """The fp16 pair of t at ``scale`` (None: per-tensor, on the device): attached by its producer (same step,
+    unmodified), else split now and memoised on t for the step (an activation feeding several convolutions, a weight
+    used by several launches, a gradient read by the dgrad and the wgrad)."""
     h = _step_get(t, '_pxl_h16')
-    if h is not None and h.has_lo >= want_lo:
+    if h is not None and h.has_lo >= want_lo and h.scale == scale:
         return h
     if getattr(t, '_pxl_carrier', False):
         raise RuntimeError('fp16-pair carrier tensor without a valid pair (stale step?)')
@@ -756,6 +762,8 @@ def conv_weight(w, form, shape, transposed=False, want_lo=True):
     (tf32 hi, lo) or 'h16' (fp16 pair at H16_W_SCALE); transposed: [Cin][T][Cout], the dgrad operand.  A weight of a
     registered parameter arena comes from the arena-wide copy (one launch per step for all weights); any other weight
     is converted here, its plain split and pair cached on the tensor for the step."""
+    if form == 'raw' and not transposed:
+        return w
     arena, off = _arena_of(w)
     if arena is not None and arena._conv_at.get(off) == shape:
         n = w.numel()
@@ -814,28 +822,28 @@ def _stride2_dgrad_classes(taps, ntaps):
 
 
 def conv_raw(x, w_packed, bias, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div, out=None, precision=None, bn_stats=None,
-             accumulate=False):
-    """Launch the NHWC tap-table convolution on raw buffers.  w_packed: [Cout][ntaps][Cin] contiguous, or the form the
-    kernel reads (tf32 split tuple, H16).  The kernel family is conv_route's choice for the shape and precision:
-    precision 0 FFMA; 1 wgmma single-pass TF32; 2 wgmma 3xTF32 (activations split in shared memory, weights here);
-    3 / 4 fp16-pair / single-fp16 wgmma.  bn_stats: the tensor-core epilogue also accumulates sum(y), sum(y^2) per
-    channel into it.  accumulate (fp16 kernels): out += the result."""
+             accumulate=False, dgrad=False):
+    """Launch the NHWC tap-table convolution on raw buffers.  x: fp32, or an fp16 pair (H16) the caller holds;
+    w_packed: [Cout][ntaps][Cin] contiguous fp32, or an H16.  The kernel family is conv_route's choice for the shape
+    and precision: precision 0 FFMA; 1 wgmma single-pass TF32; 2 wgmma 3xTF32 (activations split in shared memory,
+    weights here); 3 / 4 fp16-pair / single-fp16 wgmma (fp32 operands are split into pairs here).  dgrad: the launch
+    is the input gradient of a convolution: w_packed is that convolution's weight, stored [Cin][ntaps][Cout] in this
+    launch's terms and transposed here into the form the kernel reads, and x is its output gradient, whose pair takes
+    a per-tensor scale.  bn_stats: the tensor-core epilogue also accumulates sum(y), sum(y^2) per channel into it.  accumulate (fp16
+    kernels): out += the result."""
     ntaps = len(taps) // 2
     family, prec = conv_route('fwd', Cin, Cout, mul, div, _conv_precision if precision is None else precision)
     if family != 'h16' and (isinstance(x, H16) or isinstance(w_packed, H16)):
         raise ValueError('fp16-pair operands given for a shape the f16 wgmma kernel does not cover')
+    wshape = (Cin, ntaps, Cout) if dgrad else (Cout, ntaps, Cin)
     if out is None:
-        out = torch.empty((N, ldo, OH, OW), dtype=torch.float32, device=(x[0] if isinstance(x, tuple) else x).device,
-                          memory_format=CL)
+        out = torch.empty((N, ldo, OH, OW), dtype=torch.float32, device=x.device, memory_format=CL)
         if ldo != Cout:
             out.zero_()
     if family == 'ffma':
-        if isinstance(x, tuple):
-            x = x[0] + x[1]
-        if isinstance(w_packed, tuple):
-            w_packed = w_packed[0] + w_packed[1]
         geom = ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, div, ntaps, 0)
-        call('pxl_conv_nhwc', ctypes.byref(geom), _ctaps(taps), _p(x), _p(w_packed), _p(bias), _p(out), _stream())
+        call('pxl_conv_nhwc', ctypes.byref(geom), _ctaps(taps), _p(x), _p(conv_weight(w_packed, 'raw', wshape, dgrad)),
+             _p(bias), _p(out), _stream())
         return out
     if div == 1:
         ext = None
@@ -855,9 +863,9 @@ def conv_raw(x, w_packed, bias, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div,
                 launches.append((ConvGeom(N, H, W, Cin, ohs, ows, Cout, ldo, 1, 1, len(widx), prec), sub,
                                  ConvTcExt(ntaps, (ctypes.c_int * len(widx))(*widx), 2, py, px, OH, OW, None)))
     if family == 'h16':
-        want_lo = prec == 3
-        xh = x if isinstance(x, H16) else _pair_of(x, want_lo)
-        wh = w_packed if isinstance(w_packed, H16) else conv_weight(w_packed, 'h16', (Cout, ntaps, Cin), want_lo=want_lo)
+        want_lo = h16_has_lo(prec)
+        xh = x if isinstance(x, H16) else _pair_of(x, want_lo, None if dgrad else H16_ACT_SCALE)
+        wh = w_packed if isinstance(w_packed, H16) else conv_weight(w_packed, 'h16', wshape, dgrad, want_lo)
         fx, px = xh.inv_scale()
         fw, pw = wh.inv_scale()
         if px is not None and pw is not None:
@@ -870,14 +878,10 @@ def conv_raw(x, w_packed, bias, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div,
                         meta=(2.0 * geom.N * geom.OH * geom.OW * geom.Cin * geom.Cout * geom.ntaps,
                               'fwd/dgrad N%d %dx%d Cin%d Cout%d taps%d mul%d' % (geom.N, geom.OH, geom.OW, geom.Cin, geom.Cout, geom.ntaps, geom.mul)))
         return out
-    x_parts = x if isinstance(x, tuple) else (x, None)
-    if prec == 2:
-        w_parts = w_packed if isinstance(w_packed, tuple) else conv_weight(w_packed, 'split', (Cout, ntaps, Cin))
-    else:
-        w_parts = (w_packed, None)
+    w_parts = conv_weight(w_packed, 'split', wshape, dgrad) if prec == 2 else (conv_weight(w_packed, 'raw', wshape, dgrad), None)
     for geom, tp, ext in launches:
         _timed_call('pxl_conv_tc_launch_ex', ctypes.byref(geom), _ctaps(tp), ctypes.byref(ext) if ext is not None else None,
-                    _p(x_parts[0]), _p(x_parts[1]), _p(w_parts[0]), _p(w_parts[1]), _p(bias), _p(out), _stream(),
+                    _p(x), None, _p(w_parts[0]), _p(w_parts[1]), _p(bias), _p(out), _stream(),
                     meta=(2.0 * geom.N * geom.OH * geom.OW * geom.Cin * geom.Cout * geom.ntaps,
                           'fwd/dgrad(tf32) N%d %dx%d Cin%d Cout%d taps%d' % (geom.N, geom.OH, geom.OW, geom.Cin, geom.Cout, geom.ntaps)))
     return out
@@ -889,16 +893,17 @@ def conv_tc_status():
 
 
 def conv_wgrad_raw(x, dy, dw, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div, precision=None):
-    """dw[Cout][ntaps][Cin] += ...  (dw must be initialised by the caller)."""
+    """dw[Cout][ntaps][Cin] += ...  (dw must be initialised by the caller).  x, dy: fp32, or fp16 pairs the caller
+    holds; the fp16-pair kernels read x's pair at the fixed activation scale and dy's at a per-tensor scale."""
     ntaps = len(taps) // 2
     family, prec = conv_route('wgrad', Cin, ldo, mul, div, _conv_precision if precision is None else precision)
     if family != 'h16' and (isinstance(x, H16) or isinstance(dy, H16)):
         raise ValueError('fp16-pair operands given for a shape the f16 wgmma wgrad kernel does not cover')
     geom = ConvGeom(N, H, W, Cin, OH, OW, Cout, ldo, mul, div, ntaps, prec)
     if family == 'h16':
-        want_lo = prec == 3
-        xh = x if isinstance(x, H16) else h16_split(x, H16_ACT_SCALE, want_lo)
-        dh = dy if isinstance(dy, H16) else h16_split(dy, None, want_lo)
+        want_lo = h16_has_lo(prec)
+        xh = x if isinstance(x, H16) else _pair_of(x, want_lo)
+        dh = dy if isinstance(dy, H16) else _pair_of(dy, want_lo, None)
         fx, px = xh.inv_scale()
         fd, pd = dh.inv_scale()
         if px is not None and pd is not None:
@@ -906,21 +911,78 @@ def conv_wgrad_raw(x, dy, dw, taps, N, H, W, Cin, OH, OW, Cout, ldo, mul, div, p
         _timed_call('pxl_conv_wgrad_h16_launch', ctypes.byref(geom), _ctaps(taps), _p(xh.hi), _p(xh.lo), _p(dh.hi), _p(dh.lo),
                     _p(dw), float(fx * fd), _p(pd if pd is not None else px), _stream(),
                     meta=(2.0 * N * OH * OW * Cin * Cout * ntaps, 'wgrad N%d %dx%d Cin%d Cout%d taps%d mul%d' % (N, OH, OW, Cin, Cout, ntaps, mul)))
-    elif family == 'tc':
-        if prec == 2 and isinstance(x, tuple) != isinstance(dy, tuple):        # mixed: split the raw one too
-            x = x if isinstance(x, tuple) else split_tf32(x)
-            dy = dy if isinstance(dy, tuple) else split_tf32(dy)
-        x_hi, x_lo = x if isinstance(x, tuple) else (x, None)     # raw operands: 3xTF32 splits them inside the kernel
-        d_hi, d_lo = dy if isinstance(dy, tuple) else (dy, None)
-        _timed_call('pxl_conv_wgrad_tc_launch', ctypes.byref(geom), _ctaps(taps), _p(x_hi), _p(x_lo), _p(d_hi), _p(d_lo),
+    elif family == 'tc':      # raw operands: 3xTF32 splits them inside the kernel
+        _timed_call('pxl_conv_wgrad_tc_launch', ctypes.byref(geom), _ctaps(taps), _p(x), None, _p(dy), None,
                     _p(dw), _stream(), meta=(2.0 * N * OH * OW * Cin * Cout * ntaps, 'wgrad(tf32) N%d %dx%d Cin%d Cout%d taps%d' % (N, OH, OW, Cin, Cout, ntaps)))
     else:
-        if isinstance(x, tuple):
-            x = x[0] + x[1]
-        if isinstance(dy, tuple):
-            dy = dy[0] + dy[1]
         call('pxl_conv_wgrad_nhwc', ctypes.byref(geom), _ctaps(taps), _p(x), _p(dy), _p(dw), _stream())     # FFMA split-K
     return dw
+
+
+def conv_input(x, Cin, Cout, stride):
+    """Input x of a Cin -> Cout (output lanes) convolution in the form its wgrad reads, which is what its node keeps
+    for the backward: x's fp16 pair when the wgrad runs on the fp16-pair kernels (the forward then does too, and reads
+    the same pair), else x."""
+    family, prec = conv_route('wgrad', Cin, Cout, stride, 1, _conv_precision)
+    return _pair_of(x, h16_has_lo(prec)) if family == 'h16' else x
+
+
+def _keep(x):
+    """What ctx.save_for_backward takes of a convolution input: x, or the buffer of its activation-scale fp16 pair."""
+    return x.buf if isinstance(x, H16) else x
+
+
+def _kept(t):
+    """The convolution input that _keep(x) saved as t."""
+    if t is None or t.dtype != torch.float16:
+        return t
+    return H16(t, t.shape[1], H16_ACT_SCALE, None, h16_has_lo(_conv_precision))
+
+
+def _conv_dgrad(dy, w, taps, N, H, W, Cin, OH, OW, Cout, stride, into=None, transposed=False):
+    """dX [N, Cin, H, W] of the convolution x -> y [N, Cout, OH, OW] with ``taps`` and ``stride`` from dy: a forward
+    launch over dy with the taps negated and ``stride`` as the dgrad stride.  w: the forward's weight, transposed by the
+    launcher, or (transposed) the node's own [Cin][ntaps][Cout] packing of it.  into: dX is added into this buffer by
+    the fp16 kernels' epilogue, or after the launch where that epilogue does not apply."""
+    args = (dy, w, None, [-v for v in taps], N, OH, OW, Cout, H, W, Cin, Cin, 1, stride)
+    if into is not None:
+        try:
+            return conv_raw(*args, out=into, accumulate=True, dgrad=not transposed)
+        except _lib.PxlError as e:
+            if e.code != _lib.PXL_ERR_UNSUPPORTED:
+                raise
+    dx = conv_raw(*args, dgrad=not transposed)
+    if into is not None:
+        dx += into
+    return dx
+
+
+def _conv_wgrad(x, dy, weight, taps, N, H, W, Cin, OH, OW, Cout, ldo, stride):
+    """dW of a convolution node's ``weight``: the kernels add it straight into weight.grad when that is a contiguous
+    channels-last view (the flat gradient arena) and autograd gets None; otherwise, and always for a zero-padded output
+    (ldo > Cout), they add it into a zeroed buffer that is returned to autograd."""
+    inplace = ldo == Cout and weight.grad is not None and weight.grad.is_contiguous(memory_format=CL)
+    dw = weight.grad if inplace else torch.zeros_like(weight)
+    conv_wgrad_raw(x, dy, dw, taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, 1)
+    return None if inplace else dw
+
+
+def _bias_grad(dy, rows, C, ldo):
+    """Bias gradient: the per-channel sum of dy's first C of ldo lanes."""
+    db = torch.empty(C, dtype=torch.float32, device=dy.device)
+    call('pxl_bias_grad', _p(dy), rows, C, ldo, _p(db), 0, _stream())
+    return db
+
+
+def _with_conv_bn_sums(want, C, device, apply):
+    """out = apply(sums): when ``want`` and a tensor-core mode is on, sums is a zeroed fp64 [2*C] the conv epilogue
+    accumulates the output's per-channel sum / sum of squares into, attached to out as ``._pxl_bn_sums`` when the
+    launch filled it (bn_act then skips its statistics pass); else None."""
+    sums = _stat_zeros(2 * C, device) if want and _conv_precision != 0 else None
+    out = apply(sums)
+    if sums is not None and getattr(sums, '_pxl_filled', False):
+        out._pxl_bn_sums = sums
+    return out
 
 
 def transpose_weights(w_packed, Cout, T, Cin):
@@ -943,56 +1005,32 @@ class _Conv2d(torch.autograd.Function):
             raise ValueError('channel mismatch')
         ldo = max(out_lanes, Cout)
         OH, OW, taps = _conv_geometry(H, W, kh, kw, stride, padding, dilation)
-        ctx.h16 = None
-        ctx.meta = (taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, kh * kw, bias is not None)
-        prec = _conv_precision
-        if ldo == Cout and conv_route('fwd', Cin, Cout, stride, 1, prec)[0] == 'h16':
-            # fp16-pair path: the pair of x (4 B/element, like x itself) is what the backward keeps
-            xh = _pair_of(x, prec == 3)
-            out = conv_raw(xh, weight, bias, taps, N, H, W, Cin, OH, OW, Cout, Cout, stride, 1, bn_stats=bn_stats)
-            if conv_route('wgrad', Cin, Cout, stride, 1, prec)[0] == 'h16' or not ctx.needs_input_grad[1]:
-                ctx.save_for_backward(xh.buf, weight)
-                ctx.h16 = (xh.scale, xh.has_lo)
-            else:
-                ctx.save_for_backward(x, weight)
-            return out
+        x = conv_input(x, Cin, ldo, stride)
         out = conv_raw(x, weight, bias, taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, 1, bn_stats=bn_stats)
-        ctx.save_for_backward(x, weight)
+        ctx.save_for_backward(_keep(x) if ctx.needs_input_grad[1] else None, weight)
+        ctx.meta = (taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, kh * kw, bias is not None)
         return out
 
     @staticmethod
     def backward(ctx, dy):
         x, weight = ctx.saved_tensors
+        x = _kept(x)
         taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, T, has_bias = ctx.meta
         dy = as_cl(dy)                       # [N, ldo, OH, OW]; lanes >= Cout carry zeros
         dx = dw = db = None
-        if ctx.h16 is not None:
-            x = H16(x, x.shape[1], ctx.h16[0], None, ctx.h16[1])
-        prec = _conv_precision
-        dfamily, dprec = conv_route('dgrad', ldo, Cin, 1, stride, prec)
-        dgrad_h16 = ctx.needs_input_grad[0] and ldo == Cout and dfamily == 'h16'
-        dyin = dy
-        if dgrad_h16 or (ctx.needs_input_grad[1] and isinstance(x, H16)):
-            dyin = h16_split(dy, None, prec == 3)        # one pair of dY serves dgrad and wgrad
         if ctx.needs_input_grad[0]:
             if ldo != Cout:
+                # the dgrad of a zero-padded output reads the weight padded with zero rows to ldo
                 wp = torch.zeros((ldo, T, Cin), dtype=torch.float32, device=dy.device)
                 wp[:Cout] = weight.permute(0, 2, 3, 1).reshape(Cout, T, Cin)
-                wt = transpose_weights(wp, ldo, T, Cin)
+                dx = _conv_dgrad(dy, transpose_weights(wp, ldo, T, Cin), taps, N, H, W, Cin, OH, OW, ldo, stride,
+                                 transposed=True)
             else:
-                form = 'h16' if dgrad_h16 else 'split' if (dfamily, dprec) == ('tc', 2) else 'raw'
-                wt = conv_weight(weight, form, (Cout, T, Cin), transposed=True, want_lo=prec == 3)
-            dx = conv_raw(dyin if dgrad_h16 else dy, wt, None, [-v for v in taps], N, OH, OW, ldo, H, W, Cin, Cin, 1, stride)
+                dx = _conv_dgrad(dy, weight, taps, N, H, W, Cin, OH, OW, Cout, stride)
         if ctx.needs_input_grad[1]:
-            # the wgrad kernels add straight into weight.grad (the flat gradient arena); a zero-padded head's gradient
-            # goes through autograd
-            inplace = ldo == Cout and weight.grad is not None and weight.grad.is_contiguous(memory_format=CL)
-            dwbuf = weight.grad if inplace else torch.zeros_like(weight, memory_format=torch.preserve_format)
-            conv_wgrad_raw(x, dyin if isinstance(x, H16) else dy, dwbuf, taps, N, H, W, Cin, OH, OW, Cout, ldo, stride, 1)
-            dw = None if inplace else dwbuf
+            dw = _conv_wgrad(x, dy, weight, taps, N, H, W, Cin, OH, OW, Cout, ldo, stride)
         if has_bias and ctx.needs_input_grad[2]:
-            db = torch.empty(Cout, dtype=torch.float32, device=dy.device)
-            call('pxl_bias_grad', _p(dy), N * OH * OW, Cout, ldo, _p(db), 0, _stream())
+            db = _bias_grad(dy, N * OH * OW, Cout, ldo)
         return dx, dw, db, None, None, None, None, None
 
 
@@ -1001,13 +1039,8 @@ def conv2d(x, weight, bias=None, stride=1, padding=0, dilation=1, out_lanes=0, w
     want_bn_stats: when the tensor-core kernel runs, its epilogue also accumulates the per-channel
     sum / sum of squares of the output; they are attached to the result as ``._pxl_bn_sums`` (fp64 [2*Cout])
     and picked up by bn_act, which then skips its own statistics pass."""
-    sums = None
-    if want_bn_stats and _conv_precision != 0 and not out_lanes:
-        sums = _stat_zeros(2 * weight.shape[0], x.device)
-    out = _Conv2d.apply(x, weight, bias, int(stride), int(padding), int(dilation), int(out_lanes), sums)
-    if sums is not None and getattr(sums, '_pxl_filled', False):
-        out._pxl_bn_sums = sums
-    return out
+    return _with_conv_bn_sums(want_bn_stats and not out_lanes, weight.shape[0], x.device, lambda sums: _Conv2d.apply(
+        x, weight, bias, int(stride), int(padding), int(dilation), int(out_lanes), sums))
 
 
 class _Aspp(torch.autograd.Function):
@@ -1047,12 +1080,10 @@ class _Aspp(torch.autograd.Function):
         dy = as_cl(dy)          # [N, ldo, H, W]; lanes >= C are zero (bilinear backward zero-fills)
         dx = None
         if ctx.needs_input_grad[0]:
-            wt = transpose_weights(wp, ldo, 9 * nb, Cin)          # [Cin][36][ldo]
-            dx = conv_raw(dy, wt, None, [-v for v in taps], N, H, W, ldo, H, W, Cin, Cin, 1, 1)
+            dx = _conv_dgrad(dy, transpose_weights(wp, ldo, 9 * nb, Cin), taps, N, H, W, Cin, H, W, ldo, 1, transposed=True)
         dwp = torch.zeros((C, 9 * nb, Cin), dtype=torch.float32, device=dy.device)
         conv_wgrad_raw(x, dy, dwp, taps, N, H, W, Cin, H, W, C, ldo, 1, 1)
-        db = torch.empty(C, dtype=torch.float32, device=dy.device)
-        call('pxl_bias_grad', _p(dy), N * H * W, C, ldo, _p(db), 0, _stream())
+        db = _bias_grad(dy, N * H * W, C, ldo)
         dws = [dwp[:, 9 * i:9 * i + 9].reshape(C, 3, 3, Cin).permute(0, 3, 1, 2) for i in range(nb)]
         return (dx, None) + tuple(dws) + tuple(db for _ in range(nb))
 
@@ -1070,8 +1101,6 @@ class _AsppGemm(torch.autograd.Function):
         weights, biases = wb[:nb], wb[nb:]
         N, Cin, H, W = x.shape
         C = weights[0].shape[0]
-        prec = _conv_precision
-        want_lo = prec == 3
         ldo = max(_AsppGemm.LDO, (C + 3) // 4 * 4)
         taps = []
         for d in dilations:
@@ -1083,22 +1112,23 @@ class _AsppGemm(torch.autograd.Function):
         for i, wgt in enumerate(weights):
             _chk(wgt, 'aspp weight', cl=True)
             wq[9 * i * C:9 * (i + 1) * C] = wgt.detach().permute(2, 3, 0, 1).reshape(9 * C, Cin)    # (kh,kw,co,ci)
-        wh = h16_split(wq, H16_W_SCALE, want_lo)
+        wh = h16_split(wq, H16_W_SCALE, h16_has_lo(_conv_precision))
         bsum = biases[0]
         for b in biases[1:]:
             bsum = bsum + b
-        xh = _pair_of(x, want_lo)
-        z = conv_raw(xh, wh, None, [0, 0], N, H, W, Cin, H, W, ldz, ldz, 1, 1, precision=prec)
+        xh = conv_input(x, Cin, ldz, 1)
+        z = conv_raw(xh, wh, None, [0, 0], N, H, W, Cin, H, W, ldz, ldz, 1, 1)
         out = torch.empty((N, ldo, H, W), dtype=torch.float32, device=x.device, memory_format=CL)
         call('pxl_aspp_gather', _p(z), _p(bsum.detach().contiguous()), _p(out), N, H, W, C, ldz, ldo, _ctaps(taps), T, _stream())
-        ctx.save_for_backward(xh.buf, wq)
-        ctx.meta = (taps, N, H, W, Cin, C, ldo, ldz, nb, xh.scale, want_lo, prec)
+        ctx.save_for_backward(_keep(xh), wq)
+        ctx.meta = (taps, N, H, W, Cin, C, ldo, ldz, nb)
         return out
 
     @staticmethod
     def backward(ctx, dy):
         xbuf, wq = ctx.saved_tensors
-        taps, N, H, W, Cin, C, ldo, ldz, nb, xscale, want_lo, prec = ctx.meta
+        taps, N, H, W, Cin, C, ldo, ldz, nb = ctx.meta
+        want_lo = h16_has_lo(_conv_precision)
         dy = as_cl(dy)          # [N, ldo, H, W]; lanes >= C are zero (bilinear backward zero-fills)
         dev = dy.device
         T = 9 * nb
@@ -1111,13 +1141,10 @@ class _AsppGemm(torch.autograd.Function):
         dzh = H16(dz, n, None, slot, want_lo)
         dx = None
         if ctx.needs_input_grad[0]:
-            wt = h16_split(wq.t().contiguous(), H16_W_SCALE, want_lo)            # [Cin][ldz]
-            dx = conv_raw(dzh, wt, None, [0, 0], N, H, W, ldz, H, W, Cin, Cin, 1, 1, precision=prec)
+            dx = _conv_dgrad(dzh, wq.t().contiguous(), [0, 0], N, H, W, Cin, H, W, ldz, 1, transposed=True)
         dwq = torch.zeros((ldz, Cin), dtype=torch.float32, device=dev)
-        conv_wgrad_raw(H16(xbuf, xbuf.shape[1], xscale, None, want_lo), dzh, dwq, [0, 0], N, H, W, Cin, H, W, ldz, ldz, 1, 1,
-                       precision=prec)
-        db = torch.empty(C, dtype=torch.float32, device=dev)
-        call('pxl_bias_grad', _p(dy), N * H * W, C, ldo, _p(db), 0, _stream())
+        conv_wgrad_raw(_kept(xbuf), dzh, dwq, [0, 0], N, H, W, Cin, H, W, ldz, ldz, 1, 1)
+        db = _bias_grad(dy, N * H * W, C, ldo)
         g = dwq[:T * C].view(nb, 3, 3, C, Cin)                                   # (branch, kh, kw, co, ci)
         dws = [g[i].permute(2, 3, 0, 1) for i in range(nb)]                      # logical [C, Cin, 3, 3], CL strides
         return (dx, None) + tuple(dws) + tuple(db for _ in range(nb))
@@ -1162,46 +1189,35 @@ class _Stem(torch.autograd.Function):
             ctx.save_for_backward(img)
             return out
         if prec >= 3:
-            # fp16-pair path: the unfolded matrix is written directly as the hi / lo planes [pixels][kh]
-            want_lo = prec == 3
-            n = N * OH * OW * kh
+            # fp16-pair path: the unfolded matrix is written directly as the hi / lo planes [pixels][lanes]
+            lanes, n, want_lo = kh, N * OH * OW * kh, h16_has_lo(prec)
             buf = torch.empty((2, n), dtype=torch.float16, device=img.device)
             _timed_call(h16_entry, _p(img), _p(buf[0]), _p(buf[1] if want_lo else None), float(H16_ACT_SCALE),
                         N, H, W, OH, OW, _stream())
-            colsh = H16(buf, n, H16_ACT_SCALE, None, want_lo)
-            wp = torch.zeros((64, kh), dtype=torch.float32, device=img.device)
-            wp[:, :K] = weight.detach().permute(0, 2, 3, 1).reshape(64, K)
-            conv_raw(colsh, h16_split(wp, H16_W_SCALE, want_lo), None, [0, 0], N, OH, OW, kh, OH, OW, 64, 64, 1, 1, out=out,
-                     precision=prec, bn_stats=sums)
-            ctx.save_for_backward(buf if ctx.needs_input_grad[1] else None)
-            ctx.h16 = want_lo
-            return out
-        cols = torch.empty((N, kp, OH, OW), dtype=torch.float32, device=img.device, memory_format=CL)
-        _timed_call(fp32_entry, _p(img), _p(cols), N, H, W, OH, OW, _stream())
-        wp = torch.zeros((64, kp), dtype=torch.float32, device=img.device)
+            cols = H16(buf, n, H16_ACT_SCALE, None, want_lo)
+        else:
+            lanes = kp
+            cols = torch.empty((N, kp, OH, OW), dtype=torch.float32, device=img.device, memory_format=CL)
+            _timed_call(fp32_entry, _p(img), _p(cols), N, H, W, OH, OW, _stream())
+        wp = torch.zeros((64, lanes), dtype=torch.float32, device=img.device)
         wp[:, :K] = weight.detach().permute(0, 2, 3, 1).reshape(64, K)          # physical order of the CL weight
-        conv_raw(cols, wp, None, [0, 0], N, OH, OW, kp, OH, OW, 64, 64, 1, 1, out=out, precision=prec, bn_stats=sums)
-        ctx.save_for_backward(cols if ctx.needs_input_grad[1] else None)
+        conv_raw(cols, wp, None, [0, 0], N, OH, OW, lanes, OH, OW, 64, 64, 1, 1, out=out, precision=prec, bn_stats=sums)
+        ctx.save_for_backward(_keep(cols) if ctx.needs_input_grad[1] else None)
+        ctx.lanes = lanes
         return out
 
     @staticmethod
     def backward(ctx, dy):
         (saved,) = ctx.saved_tensors
         N, H, W, OH, OW, prec, ks = ctx.meta
-        pad, (_, kp), (_, kh) = STEM_GEOMETRIES[ks]
         K = 3 * ks * ks
         dy = as_cl(dy)
         if prec == 0 and ks == 7:
             dw = torch.empty((64, 3, 7, 7), dtype=torch.float32, device=dy.device, memory_format=CL).zero_()
             call('pxl_stem_conv7x7s2_wgrad', _p(saved), _p(dy), _p(dw), N, H, W, OH, OW, _stream())
             return None, dw, None, None
-        if prec >= 3:
-            dwp = torch.zeros((64, kh), dtype=torch.float32, device=dy.device)
-            conv_wgrad_raw(H16(saved, saved.shape[1], H16_ACT_SCALE, None, ctx.h16), dy, dwp, [0, 0], N, OH, OW, kh, OH, OW, 64, 64,
-                           1, 1, precision=prec)
-        else:
-            dwp = torch.zeros((64, kp), dtype=torch.float32, device=dy.device)
-            conv_wgrad_raw(saved, dy, dwp, [0, 0], N, OH, OW, kp, OH, OW, 64, 64, 1, 1, precision=prec)
+        dwp = torch.zeros((64, ctx.lanes), dtype=torch.float32, device=dy.device)
+        conv_wgrad_raw(_kept(saved), dy, dwp, [0, 0], N, OH, OW, ctx.lanes, OH, OW, 64, 64, 1, 1, precision=prec)
         dw = dwp[:, :K].reshape(64, ks, ks, 3).permute(0, 3, 1, 2)              # logical [64,3,ks,ks], CL strides
         return None, dw, None, None
 
@@ -1210,11 +1226,8 @@ def stem_conv(img, weight, want_bn_stats=False):
     """The stride-2 stem convolution (64 output channels) whose geometry the weight's kernel size selects: ResNet's
     7x7 pad 3 or the deep stem's first 3x3 pad 1.  want_bn_stats: like conv2d - on the tensor-core path the epilogue
     accumulates the BN sums."""
-    sums = _stat_zeros(128, img.device) if (want_bn_stats and _conv_precision != 0) else None
-    out = _Stem.apply(img.contiguous(), weight, sums, int(weight.shape[-1]))
-    if sums is not None and getattr(sums, '_pxl_filled', False):
-        out._pxl_bn_sums = sums
-    return out
+    return _with_conv_bn_sums(want_bn_stats, 64, img.device, lambda sums: _Stem.apply(
+        img.contiguous(), weight, sums, int(weight.shape[-1])))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1407,15 +1420,14 @@ class _ConvBnAct(torch.autograd.Function):
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, residual, stride, padding, dilation,
                 momentum, eps, relu, group, clamp_var, out_mode, stash_key=None, stash_role=None):
         ctx.stash = (stash_key, stash_role)
-        prec = _conv_precision
-        want_lo = prec == 3
+        want_lo = h16_has_lo(_conv_precision)
         N, Cin, H, W = x.shape
         Cout, Cin2, kh, kw = weight.shape
         if Cin2 != Cin:
             raise ValueError('channel mismatch')
         OH, OW, taps = _conv_geometry(H, W, kh, kw, stride, padding, dilation)
-        xh = _pair_of(x, want_lo)
-        dev = xh.device
+        xh = conv_input(x, Cin, Cout, stride)
+        dev = x.device
         sums = _stat_zeros(2 * Cout, dev)
         c = conv_raw(xh, weight, None, taps, N, H, W, Cin, OH, OW, Cout, Cout, stride, 1, bn_stats=sums)
         rows = N * OH * OW
@@ -1433,9 +1445,8 @@ class _ConvBnAct(torch.autograd.Function):
             _chk(residual, 'residual', cl=True)
         count = _bn_train_forward(c, sums, rows, Cout, gamma, beta, running_mean, running_var, momentum, eps, clamp_var,
                                   group, coeff, residual, relu, y, (_p(hi), _p(lo), float(H16_ACT_SCALE), _p(mask)))
-        ctx.save_for_backward(xh.buf, weight, c, mask, gamma, coeff, beta)
-        ctx.meta = (taps, N, H, W, Cin, OH, OW, Cout, stride, kh * kw, count, bool(relu), residual is not None, group,
-                    xh.scale, want_lo, prec)
+        ctx.save_for_backward(_keep(xh), weight, c, mask, gamma, coeff, beta)
+        ctx.meta = (taps, N, H, W, Cin, OH, OW, Cout, stride, count, bool(relu), residual is not None, group)
         out = pair.view(torch.float32).view(N, OH, OW, Cout).permute(0, 3, 1, 2) if out_mode == 'pair' else y
         if pair is not None:
             _attach_pair(out, H16(pair, n, H16_ACT_SCALE, None, want_lo), carrier=out_mode == 'pair')
@@ -1444,13 +1455,14 @@ class _ConvBnAct(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         xbuf, weight, c, mask, gamma, coeff, beta = ctx.saved_tensors
-        taps, N, H, W, Cin, OH, OW, Cout, stride, T, count, relu, has_res, group, xscale, want_lo, prec = ctx.meta
+        taps, N, H, W, Cin, OH, OW, Cout, stride, count, relu, has_res, group = ctx.meta
         if is_carrier(dy):
             raise RuntimeError('gradient tensors are never fp16-pair carriers')
         if relu and has_res and mask is None:
             raise RuntimeError('the ReLU mask of a residual unit was not recorded in the forward')
         dh, dres, dgamma, dbeta = _bn_backward(c, as_cl(dy), coeff, gamma, beta, count, N * OH * OW, Cout, relu, group,
-                                               mask=mask, want_dres=has_res, dx_pair=True, want_lo=want_lo)
+                                               mask=mask, want_dres=has_res, dx_pair=True,
+                                               want_lo=h16_has_lo(_conv_precision))
         dx = dw = None
         stash_key, stash_role = ctx.stash
         if stash_role == 'give' and dres is not None:
@@ -1460,21 +1472,10 @@ class _ConvBnAct(torch.autograd.Function):
             dres = None
         give_dx = stash_role == 'give_dx' and _residual_stash.get(stash_key) is None
         if ctx.needs_input_grad[0]:
-            wt = conv_weight(weight, 'h16', (Cout, T, Cin), transposed=True, want_lo=want_lo)
             held = _residual_stash.pop(stash_key, None) if stash_role == 'take' else None
             if stash_role == 'take' and held is None:
                 _residual_stash[stash_key] = 'taken'          # a 'give_dx' unit that runs later returns its dX itself
-            if held is not None:
-                try:
-                    dx = conv_raw(dh, wt, None, [-v for v in taps], N, OH, OW, Cout, H, W, Cin, Cin, 1, stride, out=held,
-                                  precision=prec, accumulate=True)
-                except _lib.PxlError as e:
-                    if e.code != _lib.PXL_ERR_UNSUPPORTED:
-                        raise
-                    dx = conv_raw(dh, wt, None, [-v for v in taps], N, OH, OW, Cout, H, W, Cin, Cin, 1, stride, precision=prec)
-                    dx += held
-            else:
-                dx = conv_raw(dh, wt, None, [-v for v in taps], N, OH, OW, Cout, H, W, Cin, Cin, 1, stride, precision=prec)
+            dx = _conv_dgrad(dh, weight, taps, N, H, W, Cin, OH, OW, Cout, stride, into=held)
         elif stash_role == 'take':
             _residual_stash.pop(stash_key, None)
         if give_dx and dx is not None:
@@ -1483,11 +1484,7 @@ class _ConvBnAct(torch.autograd.Function):
             _residual_stash[stash_key] = dx
             dx = None
         if ctx.needs_input_grad[1]:
-            inplace = weight.grad is not None and weight.grad.is_contiguous(memory_format=CL)
-            dwbuf = weight.grad if inplace else torch.zeros_like(weight, memory_format=torch.preserve_format)
-            conv_wgrad_raw(H16(xbuf, xbuf.shape[1], xscale, None, want_lo), dh, dwbuf, taps, N, H, W, Cin, OH, OW, Cout, Cout,
-                           stride, 1, precision=prec)
-            dw = None if inplace else dwbuf
+            dw = _conv_wgrad(_kept(xbuf), dh, weight, taps, N, H, W, Cin, OH, OW, Cout, Cout, stride)
         return (dx, dw, dgamma, dbeta, None, None, dres) + (None,) * 11
 
 
@@ -1583,7 +1580,7 @@ class _DwBnPair(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, stride, dilation, momentum, eps, group, clamp_var):
-        want_lo = _conv_precision == 3
+        want_lo = h16_has_lo(_conv_precision)
         c, meta = _dw_forward(x, weight, stride, dilation)
         N, ld, H, W, C, OH, OW = meta[:7]
         rows, dev = N * OH * OW, x.device
